@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — headline measurement of the hot path (contract in the task statement / DESIGN.md §Measurement).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 Metric: rollout tokens/s (the reference's actor/output_tokens_per_second, pipelinerl/actor.py:98-106) of the
 sampler's token step on random-init Qwen2.5-7B: 64 running sequences per GPU (actor.llm_max_rollouts,
@@ -18,8 +18,13 @@ rollouts with) in a subprocess on the same box.
 
 ONE JSON line on stdout (rank 0).  Extra keys: roofline (dominant kernel = paged decode attention),
 cpu_baseline (oracle port on the host cores, bounded sample), components (trainer side: fused AdamW and PG-loss
-tail on 7B-sized inputs, and `trainer_step` = hot path 2 end to end on Qwen2.5-7B: 2 x 16 384-token micro-batches
-through rl_step -> native backward -> fused AdamW; tools/train_bench.py).
+tail on 7B-sized inputs, and `trainer_step` = hot path 2 end to end on Qwen2.5-1.5B -- 7B's fp32 optimizer state
+alone exceeds one 80 GB H100 -- : 2 x 16 384-token micro-batches through rl_step -> native backward -> fused AdamW;
+tools/train_bench.py).
+
+--dump-outputs DIR writes what the timed token step returned in its LAST timed step, as a caller of the step receives
+it: DIR/sampled_ids.npy (float64, exact token ids) and DIR/sampled_logprobs.npy (float32), one row per sequence.  Every
+input is generated from fixed seeds, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -55,7 +60,10 @@ def parse():
     ap.add_argument("--no-vllm", action="store_true", help="N = 1: skip the vLLM 0.22 A/B subprocess")
     ap.add_argument("--no-seq-parallel", action="store_true", help="N = 2: skip the sequence-parallel trainer step")
     ap.add_argument("--no-rollout", action="store_true", help="N = 1: skip the full-rollout run through the plugin API")
-    ap.add_argument("--rollout-tokens", type=int, default=8192, help="max_tokens of the full-rollout component")
+    ap.add_argument("--rollout-tokens", type=int, default=4096,
+                    help="max_tokens of the full-rollout component (64 x (8192 + 4096) tokens of KV cache fit an 80 GB H100)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's sampled ids and logprobs as .npy files into DIR")
     ap.add_argument("--splits", default="", help="learner counts of the split runs, e.g. '2,4' (default: by N)")
     return ap.parse_args()
 
@@ -104,24 +112,12 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def ncu_traffic_bytes(algorithmic_bytes: int):
-    """DRAM bytes per launch of the dominant kernel from the committed `ncu --set full` capture
-    (profiles/r1_attn_full_raw.csv: dram__bytes_read.sum 1.08266 GB + dram__bytes_write.sum 0.9 MB at B=64, S=8240 -> ratio
-    to the algorithmic bytes 1.0004), scaled to the bytes of the launch timed here."""
-    f = ROOT / "profiles" / "ncu_traffic.json"
-    try:
-        ratio = float(json.loads(f.read_text())["paged_attn_decode_kernel"]["traffic_over_algorithmic"])
-    except Exception:  # noqa: BLE001
-        return None
-    return int(algorithmic_bytes * ratio)
-
-
 def measured_peaks():
     f = ROOT / "MEASURED_PEAKS.json"
     if f.exists():
         d = json.loads(f.read_text())
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
 # ----------------------------------------------------------------------------------------------
@@ -162,6 +158,15 @@ def algorithmic_bytes(cfg, B, S):
     w_head = (4 if cfg.fp32_head else 2) * cfg.vocab_size * cfg.hidden_size   # hi + lo streams = an fp32 weight's bytes
     kv_per_layer = B * S * 2 * cfg.num_kv_heads * cfg.head_dim * 2
     return w_body + w_head, kv_per_layer
+
+
+def dump_outputs(out_dir: str, eng) -> None:
+    """The token step's outputs of the step that just ran: sampled token ids and their logprobs, one per sequence."""
+    import numpy as np
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    np.save(d / "sampled_ids.npy", eng.sampled.detach().cpu().numpy().astype(np.float64))
+    np.save(d / "sampled_logprobs.npy", eng.sampled_lp.detach().cpu().numpy().astype(np.float32))
 
 
 def run_ours(args):
@@ -212,6 +217,8 @@ def run_ours(args):
     barrier()
     ms = ev0.elapsed_time(ev1)
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng)
 
     # ---- end-to-end through the host-facing call: token ids in from pinned host memory, ids + logprobs out ----
     h_tok = torch.zeros(eng.B, dtype=torch.int32).pin_memory()
@@ -267,8 +274,6 @@ def run_ours(args):
     step_bytes = w_bytes + cfg.num_layers * kv_bytes
     roofline = {"kernel": "paged_attn_decode_kernel(+combine)", "bound": "hbm", "achieved": round(achieved, 1),
                 "peak": peak, "peak_source": peak_src, "unit": "GB/s", "frac": round(achieved / peak, 4),
-                "traffic": ncu_traffic_bytes(kv_bytes), "traffic_source": "ncu --set full dram__bytes_read.sum + "
-                "dram__bytes_write.sum of this kernel (profiles/r1_attn_full_raw.csv: read 1.0004 x, read+write 1.0046 x algorithmic), scaled to this launch",
                 "launch_ms": round(attn_ms, 4), "algorithmic_bytes_per_launch": kv_bytes,
                 "share_of_step": round(attn_ms * cfg.num_layers / (ms / args.steps), 4),
                 "whole_step": {"algorithmic_bytes": step_bytes,
@@ -293,11 +298,12 @@ def run_ours(args):
         del eng, attn_all_layers
         gc.collect()
         torch.cuda.empty_cache()
-        out["components"]["trainer_step"] = run_tool(["tools/train_bench.py", "--steps", "2", "--warmup", "1"], 600)
+        out["components"]["trainer_step"] = run_tool(["tools/train_bench.py", "--model", "1.5b", "--steps", "2", "--warmup", "1"],
+                                                     600)
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
         out["cpu_baseline"] = cpu_baseline(args, budget_s=25.0)
     if rank == 0 and world == 1 and not args.no_components and not args.no_rollout:
-        # whole rollouts through the plugin API: prefill + decode growing 8192 -> 16384 (not a static-state microbench)
+        # whole rollouts through the plugin API: prefill + decode growing from the 8192-token prompt (not a static-state microbench)
         out["components"]["rollout_full"] = run_tool(["tools/rollout_bench.py", "--max-tokens", str(args.rollout_tokens)], 600)
     if rank == 0 and world == 1 and not args.no_components and not args.no_vllm:
         out.setdefault("components", {})["vllm_baseline"] = vllm_baseline(args)
@@ -416,7 +422,7 @@ def run_tool(argv, timeout_s):
 
 
 def vllm_baseline(args):
-    """Same workload on vLLM 0.22 + FlashInfer sm_100 (the engine family the reference serves rollouts with; it pins
+    """Same workload on vLLM 0.22 + FlashInfer (the engine family the reference serves rollouts with; it pins
     0.18.1) on this box, in a subprocess (tools/vllm_baseline.py): a LIBRARY baseline for the A/B, not product code."""
     import gc
     import torch

@@ -1,5 +1,5 @@
 /*
- * prl.h — C ABI of libprl.so, the B200 (sm_100a) hot-path library behind the
+ * prl.h — C ABI of libprl.so, the H100 (sm_90a) hot-path library behind the
  * PipelineRL plugin / stream API.
  *
  * Conventions (SURVEY.md §8b):
@@ -164,7 +164,7 @@ int prl_logprob_rows_bwd(const float* logits, int64_t n_rows, int64_t V, int64_t
                          const int64_t* targets /*[n_rows]*/, float temperature, const float* lse,
                          const float* entropy, const float* g_logprobs, const float* g_entropy,
                          float* dlogits, int64_t dlogits_stride, prl_stream_t stream);
-/* Backward of the fused head WITHOUT materialised logits: one GEMM (X W_hi^T + X W_lo^T in TMEM, as prl_head_logprob) whose
+/* Backward of the fused head WITHOUT materialised logits: one GEMM (X W_hi^T + X W_lo^T accumulated together, as prl_head_logprob) whose
  * epilogue writes dz[M, ld_dz] bf16 = inv_T * (g_lp * (onehot(target) - p) - g_ent * p * (log p + H)), p = exp(z / T - lse):
  * the operand of the dX / dW GEMMs.  Replaces logits GEMM(s) -> prl_logprob_rows_bwd -> bf16 cast (autograd through
  * rl/__init__.py:207-233).  lse / entropy: the forward's outputs; g_logprobs / g_entropy may be NULL. */
@@ -274,9 +274,9 @@ int prl_preprocess_pack(const prl_mb_record* record, int32_t divide_advantage_by
                         const prl_mb_columns* out, void* workspace, size_t workspace_bytes, prl_stream_t stream);
 
 /* ======================================================================= *
- * Hot path (1): tcgen05 weight-streaming GEMM of the token step
+ * Hot path (1): wgmma weight-streaming GEMM of the token step
  *   Y[M, N] = X[M, K] * W[N, K]^T, bf16 operands (row-major, K contiguous),
- *   fp32 accumulation in TMEM.  Replaces the cuBLAS GEMMs the vLLM engine runs
+ *   fp32 accumulation in registers.  Replaces the cuBLAS GEMMs the vLLM engine runs
  *   per decode step for the reference (pipelinerl/async_llm.py:134 ->
  *   /v1/chat/completions; flags conf/base.yaml:59-73) and, with W_lo, the fp32
  *   lm_head matmul of pipelinerl/vllm_quantization.py:266-278
@@ -290,15 +290,12 @@ int prl_gemm_set_smem_budget_kb(int32_t kb);
 /* Weight layout switch: 0 = row-major [N,K]; 1 = contiguous 16 KB tiles [N/128][K/64][128][64] (one sequential
  * TMA box per tile; needs N % 128 == 0, K % 64 == 0). */
 int prl_gemm_set_tiled_weights(int32_t on);
-/* M_tok > 128 (chunked prefill / scoring / learner shapes): 1 (default) = CTA-pair kernel, one
- * tcgen05.mma.cta_group::2 256x256 tile per (2,1,1) cluster; 0 = the single-CTA 128x256 kernel. */
-int prl_gemm_set_cta_pair(int32_t on);
 /* Compute-bound GEMM of the learner body / prefill (csrc/gemm_tn.cu), replaces the cuBLAS GEMMs under the HF
  * Qwen2 forward+backward that rl_step drives (pipelinerl/finetune/rl/__init__.py:190-207, finetune_loop.py:716-725):
  *     C[M,N] (=|+=) alpha * A[M,K] * B[N,K]^T (+ bias[N]) (+ residual[M,N])
  * A, B bf16 row-major with row strides lda / ldb (elements, multiples of 8, base 16-byte aligned); C bf16 or fp32
- * (c_is_f32), `accumulate` (fp32 only) adds into C; bias / residual bf16 or NULL.  Persistent CTA-pair kernel
- * (tcgen05.mma.cta_group::2, 256x256 tiles, double-buffered TMEM accumulators). */
+ * (c_is_f32), `accumulate` (fp32 only) adds into C; bias / residual bf16 or NULL.  One CTA per 128x256 output tile
+ * (TMA operand ring, two wgmma m64n256 warpgroups, fp32 accumulators in registers). */
 int prl_gemm_tn(const void* A, int64_t lda, const void* B, int64_t ldb, int64_t M, int64_t N, int64_t K,
                 void* C, int64_t ldc, int32_t c_is_f32, int32_t accumulate, const void* bias,
                 const void* residual, int64_t ldr, float alpha, prl_stream_t stream);
@@ -365,7 +362,7 @@ int prl_gemm_swiglu_decode(const void* W_bf16, const void* X_bf16, int64_t M, in
                            prl_stream_t stream);
 
 /* Fused output head with IN-KERNEL logprob capture: logits = X W^T (+ W_lo) are produced tile by tile in
- * TMEM and reduced on the spot — per token logsumexp, exact entropy, the log-probability of a given target
+ * registers and reduced on the spot — per token logsumexp, exact entropy, the log-probability of a given target
  * (teacher forcing: the trainer's new_logprobs, rl/__init__.py:207-233, and the reference-logprob scoring of
  * llm.py:606-648) and/or a sample from softmax(logits/T) with its log-probability (the sampler +
  * processed_logprobs path, conf/base.yaml:65).  Full-vocabulary logits (608 KB/token in fp32 for Qwen2.5)
@@ -425,8 +422,8 @@ int prl_paged_attn_prefill(const void* q_bf16 /*[rows,n_q,128]*/, const void* kv
                            const int32_t* seq_slot, int32_t n_seqs, int32_t max_q_len, int32_t n_q, int32_t n_kv,
                            int32_t head_dim, int32_t page_size, float sm_scale, void* out_bf16 /*[rows,n_q*128]*/,
                            prl_stream_t stream);
-/* Same contract on the tcgen05 path (csrc/attn_tc.cu): a query tile packs 128 / (n_q / n_kv) tokens x the GQA group's
- * heads into one UMMA tile, S = Q K^T and P V run on the tensor core with TMEM accumulators, V is read as stored
+/* Same contract on the wgmma path (csrc/attn_tc.cu): a query tile packs 128 / (n_q / n_kv) tokens x the GQA group's
+ * heads into 128 rows, S = Q K^T and P V run on the tensor core with register accumulators, V is read as stored
  * (MN-major operand).  q_rows = rows of the q buffer that hold this chunk (TMA bounds). */
 int prl_paged_attn_prefill_tc(const void* q_bf16 /*[q_rows,n_q,128]*/, int32_t q_rows, const void* kv_cache_bf16,
                               int64_t n_pages, int32_t n_layers, int32_t layer, const int32_t* block_table,
@@ -442,17 +439,17 @@ int prl_paged_attn_prefill_tc(const void* q_bf16 /*[q_rows,n_q,128]*/, int32_t q
  * fwd: out [T, n_q*128] bf16, lse [T, n_q] fp32 (log2 domain of the scaled scores; NULL = not needed).
  * bwd: dqkv [T, dqkv_stride] bf16 in the layout of qkv (every segment row is written); dK / dV are reduced over
  * the GQA group inside the tensor core in a fixed order (deterministic, no atomics).
- * csrc/attn_tc.cu (forward) and csrc/attn_train.cu (backward): tcgen05 MMAs, TMEM accumulators, TMA operands. */
+ * csrc/attn_tc.cu (forward) and csrc/attn_bwd.cu (backward): wgmma, register accumulators, TMA operands. */
 int prl_attn_varlen_fwd(const void* qkv_bf16, int64_t qkv_stride, int32_t T, const int32_t* seg_start,
                         const int32_t* seg_len, int32_t n_seg, int32_t max_seg_len, int32_t n_q, int32_t n_kv,
                         int32_t head_dim, float sm_scale, void* out_bf16, float* lse, prl_stream_t stream);
-/* which forward kernel prl_attn_varlen_fwd launches: 2 (default) = two ping-pong softmax groups, O accumulated in TMEM
- * with conditional rescale; 1 = the first-generation kernel shared with chunked prefill.  For A/B runs and tests. */
+/* which forward kernel prl_attn_varlen_fwd / _fwd_kv launch: 2 (default) = O and the row sum rescaled only when a row's maximum
+ * grew by more than 2^8 since its reference exponent was set; 1 = rescaled at every step. */
 int prl_attn_set_fwd_generation(int32_t generation);
 /* same switch for prl_paged_attn_prefill_tc (chunked prefill / scoring): default 2 */
 int prl_attn_set_prefill_generation(int32_t generation);
-/* backward kernels: 2 (default) = P^T / dS^T / dS reach the tensor core through TMEM (A operand in tensor memory);
- * 1 = through shared memory.  For A/B runs and tests. */
+/* backward kernels: how P^T / dS^T (dK/dV kernel) and dS (dQ kernel) reach the tensor core -- 2 (default) = register operands in
+ * both, 1 = through shared memory in both, 3 = registers in dK/dV and shared memory in dQ, 4 = the reverse.  Same bits. */
 int prl_attn_set_bwd_generation(int32_t generation);
 size_t prl_attn_varlen_bwd_workspace_bytes(int32_t T, int32_t n_q);
 int prl_attn_varlen_bwd(const void* qkv_bf16, int64_t qkv_stride, int32_t T, const int32_t* seg_start,
@@ -477,18 +474,6 @@ int prl_attn_varlen_bwd_kv(const void* q_bf16, int64_t q_stride, int32_t Tq, con
                            int32_t n_q, int32_t n_kv, int32_t head_dim, float sm_scale, const void* out_bf16,
                            const void* d_out_bf16, const float* lse, void* dq_bf16, int64_t dq_stride, void* dkv_bf16,
                            int64_t dkv_stride, void* workspace, size_t workspace_bytes, prl_stream_t stream);
-/* Measurement helper (tools/attn_bench.py --tmem): cycles for `warps` warps of every SM to read iters x 4 KB out of
- * TMEM with tcgen05.ld.32x32b.x32; out3 = {cycles, bytes per SM, -}. */
-int prl_debug_tmem_read_bench(int32_t iters, int32_t warps, int64_t* out3_device, prl_stream_t stream);
-/* measurement helper: tcgen05.mma throughput per operand configuration (modes 0-9, batches of 8 UMMAs under one lane
- * election) and the softmax <-> tensor-core hand-off round trip (mode 10); out2_device[0] = cycles, [1] = UMMAs issued
- * (profiles/r2_attention.md) */
-/* measurement helper: per-phase cycle sums of one CTA of the generation-2 learner attention forward (20 int64; NULL = off) */
-int prl_attn_debug_timing(int64_t* out20_device);
-/* likewise for the generation-4 dQ backward kernel (16 int64; NULL = off) */
-int prl_attn_debug_bwd_timing(int64_t* out16_device);
-int prl_attn_debug_bwd_timing_dkdv(int64_t* out16_device);
-int prl_debug_mma_bench(int32_t mode, int32_t iters, int64_t* out2_device, prl_stream_t stream);
 /* Sampling with in-kernel logprob capture: id ~ softmax(logits/T) (Gumbel-max, counter-based RNG on
  * (seed, step, row, vocab id)) or argmax when greedy; logprob = log_softmax(logits/T)[id]. */
 size_t prl_sample_workspace_bytes(int32_t B);

@@ -1,6 +1,6 @@
-"""In-tree build of libprl.so (hand-written sm_100a CUDA behind the C ABI in include/prl.h).
+"""In-tree build of libprl.so (hand-written sm_90a CUDA behind the C ABI in include/prl.h).
 
-nvcc cross-compiles for sm_100a without a GPU.  The .so is written next to the
+nvcc cross-compiles for sm_90a without a GPU.  The .so is written next to the
 package (pipelinerl_b200/_lib/libprl.so) so that it travels to the GPU box with
 the repository snapshot; it is git-ignored, never pip-installed.
 """
@@ -22,7 +22,7 @@ OBJ_DIR = LIB_DIR / "obj"
 LIB_PATH = LIB_DIR / "libprl.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function",
@@ -71,7 +71,7 @@ def _compile_one(src: Path, verbose: bool) -> tuple[Path, bool]:
 
 
 def build(force: bool = False, verbose: bool = True) -> Path:
-    """Compile every csrc/*.cu for sm_100a and link pipelinerl_b200/_lib/libprl.so."""
+    """Compile every csrc/*.cu for sm_90a and link pipelinerl_b200/_lib/libprl.so."""
     OBJ_DIR.mkdir(parents=True, exist_ok=True)
     if force:
         for f in OBJ_DIR.glob("*.sha"):
@@ -86,7 +86,7 @@ def build(force: bool = False, verbose: bool = True) -> Path:
     if changed:
         tmp = LIB_DIR / "libprl.so.tmp"
         cmd = [_nvcc(), "-shared", "-o", str(tmp), *map(str, objs),
-               "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC"]
+               "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC"]
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:
             sys.stderr.write(res.stdout + res.stderr)

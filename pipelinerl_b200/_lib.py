@@ -127,7 +127,6 @@ _SIGNATURES = {
     "prl_gemm_auto_split_k": (C.c_int, [C.c_int64, C.c_int64, C.c_int64]),
     "prl_gemm_set_smem_budget_kb": (C.c_int, [C.c_int32]),
     "prl_gemm_set_tiled_weights": (C.c_int, [C.c_int32]),
-    "prl_gemm_set_cta_pair": (C.c_int, [C.c_int32]),
     "prl_gemm_tn": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
                               C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,
                               C.c_float, C.c_void_p]),
@@ -170,11 +169,6 @@ _SIGNATURES = {
     "prl_attn_set_fwd_generation": (C.c_int, [C.c_int32]),
     "prl_attn_set_bwd_generation": (C.c_int, [C.c_int32]),
     "prl_attn_set_prefill_generation": (C.c_int, [C.c_int32]),
-    "prl_debug_tmem_read_bench": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
-    "prl_attn_debug_timing": (C.c_int, [C.c_void_p]),
-    "prl_attn_debug_bwd_timing": (C.c_int, [C.c_void_p]),
-    "prl_attn_debug_bwd_timing_dkdv": (C.c_int, [C.c_void_p]),
-    "prl_debug_mma_bench": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "prl_attn_varlen_bwd_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
     "prl_attn_varlen_fwd_kv": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,

@@ -22,7 +22,7 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kVec = 4;                         // elements per thread per iteration
 constexpr int kChunk = kThreads * kVec * 4;     // 4096 elements per block iteration
-constexpr int kMaxNormBlocks = 148 * 8;
+constexpr int kMaxNormBlocks = 132 * 8;
 
 struct AdamWorkspace {
   double partial[kMaxNormBlocks];

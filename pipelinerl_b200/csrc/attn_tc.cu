@@ -1,25 +1,21 @@
-// tcgen05 chunked-prefill attention (hot path 1: the <= 1024-token prefill chunks vLLM interleaves with decode,
-// conf/base.yaml:64,72; also prefix-shared prefill and reference-logprob scoring).
+// wgmma chunked-prefill attention (hot path 1: the <= 1024-token prefill chunks vLLM interleaves with decode,
+// conf/base.yaml:64,72; also prefix-shared prefill and reference-logprob scoring) and the learner's varlen forward.
 //
 // One CTA per (query tile, kv head, sequence).  A query tile packs nq = 128 / R consecutive query tokens x the R
-// query heads of one GQA group into the 128 rows of a UMMA tile (row = token * R + head), so every K/V page staged
-// by TMA serves all R heads.  Per 128-key step:
-//     S[128 x 128]  = Q K^T      tcgen05.mma, both operands K-major (k = head dim), accumulator in TMEM
-//     P             = exp2(S * scale - rowmax)   eight softmax warps, straight out of TMEM (one read);
-//                                                bf16 P goes to shared memory in the 128-byte-swizzled K-major layout
-//     Ot[128 x 128] = P V        tcgen05.mma, A = P (smem), B = V read AS STORED (MN-major operand: keys are rows)
-// and the softmax warps fold Ot into their fp32 register accumulator with the online-softmax rescale.  S and Ot are
-// double-buffered in the 512 TMEM columns and P in shared memory: the tensor core runs Q K^T of step i+1 and P V of
-// step i while the softmax warps exponentiate step i+1 / fold step i-1 (the exp phase is MUFU-bound: 16 K exp2 per
-// step against 16 per clock and SM).  Warp roles: 0 = TMA producer, 1 = MMA issuer + TMEM owner,
-// 2..9 = softmax / epilogue (two warps per TMEM lane quarter, each owning half of the keys / head-dim columns).
+// query heads of one GQA group into 128 rows (row = token * R + head), so every K/V page staged by TMA serves all R
+// heads.  Two consumer warpgroups own 64 rows each; per 128-key step a warpgroup runs
+//     S[64 x 128]  = Q K^T      wgmma, both operands K-major from shared memory (k = head dim), fp32 in registers
+//     P            = exp2(S * scale - rowmax)   online softmax in registers (rows split over the 4 lanes of a quad)
+//     O[64 x 128] += P V        wgmma with A = P straight from registers (bf16), B = V read AS STORED (MN-major)
+// and rescales O in registers when the running maximum grows.  A TMA producer warp streams K/V pages through a
+// 3-stage ring; the two warpgroups run independently, so one's softmax overlaps the other's tensor-core work.
 //
-// That is GENERATION 1 (attn_prefill_tc_kernel).  The default for both entry points is generation 2 (attn_fwd_v2_kernel,
-// further down): two softmax groups in ping-pong, P and O in TMEM.  In both, the MMA warp runs converged and elects one lane
-// per batch of UMMAs (tc_ptx.cuh: elect_one).
+// Two generations (prl_attn_set_fwd_generation / prl_attn_set_prefill_generation): 1 rescales O and the row sum at every
+// step by exp2(m_old - m_new); 2 (default) keeps a per-row REFERENCE exponent and rescales only when the row maximum has
+// grown by more than 2^8 since it was set -- P stays below 256 (exact range of bf16), and for trained or random scores the
+// 64 multiplies per thread and step are skipped after the first steps of a row.
 //
 // Tensor-bound: 4 * 128 * S^2 / 2 FLOP per head (causal); K/V bytes are re-read from L2 by the other query tiles.
-#include <stdlib.h>
 #include "prl_common.cuh"
 #include "tc_ptx.cuh"
 
@@ -31,7 +27,10 @@ constexpr int kDT = 128;
 constexpr int kKeys = 128;                 // keys per step = 2 pages
 constexpr int kTile16K = 16384;            // one [128 rows x 128 B] operand tile
 constexpr int kStageBytesT = 4 * kTile16K; // K lo/hi + V lo/hi
-constexpr int kThreadsT = 320;           // TMA warp, MMA warp, 8 softmax warps
+constexpr int kStagesT = 3;
+constexpr int kThreadsT = 288;             // 2 consumer warpgroups + TMA producer warp
+constexpr int kSmemT = 2 * kTile16K + kStagesT * kStageBytesT + 1024 + 8 * (2 * kStagesT + 1) + 16;
+static_assert(kSmemT <= 232448, "attention forward exceeds the 227 KB shared-memory limit");
 
 struct TcPrefillParams {
   __nv_bfloat16* out;            // [rows, n_q*128]
@@ -50,7 +49,6 @@ struct TcPrefillParams {
   // sequence z covers rows [seq_q_start[z], seq_q_start[z] + seq_q_len[z]) and its keys are those same rows
   int col_k, col_v;              // element column of K / V head 0
   float* lse;                    // [rows, n_q] log2-domain log-sum-exp of the scaled scores (may be NULL)
-  long long* timing;             // measurement only (prl_attn_debug_timing): per-phase cycle sums of one CTA, else NULL
 };
 
 __device__ __forceinline__ float ex2(float x) {
@@ -58,614 +56,224 @@ __device__ __forceinline__ float ex2(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ float max3(float a, float b, float c) {
-  float y;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(y) : "f"(a), "f"(b), "f"(c));
-  return y;
-}
 __device__ __forceinline__ uint32_t pack2(float a, float b) {
   const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<const uint32_t*>(&h);
 }
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+
+template <bool kContig, bool kLazyRescale>
+__global__ void __launch_bounds__(kThreadsT, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_kv, TcPrefillParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t q_smem = base;                          // Q lo | Q hi
+  const uint32_t kv_smem = base + 2 * kTile16K;          // kStagesT x (K lo | K hi | V lo | V hi)
+  const uint32_t bar_base = kv_smem + kStagesT * kStageBytesT;
+  auto full_bar = [&](int s) { return bar_base + 8u * (uint32_t)s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (uint32_t)(kStagesT + s); };
+  const uint32_t q_bar = bar_base + 8u * (uint32_t)(2 * kStagesT);
+
+  // packed training rows are long and causal: walk the query tiles heaviest-first
+  const int qtile = kContig ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
+  const int kvh = blockIdx.y, z = blockIdx.z;
+  const int q_len = p.seq_q_len[z];
+  const int pos0 = (kContig && p.seq_pos0 == nullptr) ? 0 : p.seq_pos0[z];
+  const int t0 = qtile * p.nq;
+  if (t0 >= q_len) return;                               // uniform across the CTA, before any barrier
+  const int row0 = p.seq_q_start[z] + t0;
+  const int pos_first = pos0 + t0;
+  const int n_valid = (q_len - t0) < p.nq ? (q_len - t0) : p.nq;
+  const int kv_end = pos_first + n_valid;                // keys [0, kv_end) can be visible to this tile
+  const int n_it = (kv_end + kKeys - 1) / kKeys;
+  const int last_page = (kv_end - 1) / kPageT;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 256) {
+    for (int s = 0; s < kStagesT; ++s) {
+      ptx::mbar_init(full_bar(s), 1);
+      ptx::mbar_init(empty_bar(s), 2);   // one elected thread of each consumer warpgroup
+    }
+    ptx::mbar_init(q_bar, 1);
+    ptx::fence_barrier_init();
+    ptx::fence_proxy_async();
+    ptx::prefetch_tensormap(&tm_q);
+    ptx::prefetch_tensormap(&tm_kv);
+  }
+  __syncthreads();
+
+  if (warp == 8) {
+    // ===== TMA producer =====
+    if (lane == 0) {
+      ptx::mbar_arrive_expect_tx(q_bar, (uint32_t)(2 * 128 * p.R * p.nq));
+      ptx::tma_load_3d(q_smem, &tm_q, 0, kvh * p.R, row0, q_bar, ptx::kEvictFirst);
+      ptx::tma_load_3d(q_smem + kTile16K, &tm_q, 64, kvh * p.R, row0, q_bar, ptx::kEvictFirst);
+      const int32_t* bt = kContig ? nullptr : p.block_table + (int64_t)p.seq_slot[z] * p.max_blocks;
+      const int seq_row0 = (kContig && p.seq_kv_start != nullptr) ? p.seq_kv_start[z] : p.seq_q_start[z];
+      for (int it = 0; it < n_it; ++it) {
+        const int s = it % kStagesT;
+        ptx::mbar_wait(empty_bar(s), (uint32_t)(((it / kStagesT) & 1) ^ 1));
+        ptx::mbar_arrive_expect_tx(full_bar(s), (uint32_t)kStageBytesT);
+#pragma unroll
+        for (int kv = 0; kv < 2; ++kv) {
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            int pg = 2 * it + half;
+            if (pg > last_page) pg = last_page;          // the tail step re-reads the last page; its keys are masked
+            int row, c0;
+            if (kContig) {                               // rows past the sequence / past T: masked keys (TMA zero-fills OOB)
+              row = seq_row0 + pg * kPageT;
+              c0 = (kv ? p.col_v : p.col_k) + kvh * kDT;
+            } else {
+              const int page = bt[pg];
+              row = (int)(((((int64_t)p.layer * 2 + kv) * p.n_pages + page) * p.n_kv + kvh) * kPageT);
+              c0 = 0;
+            }
+            const uint32_t dst = kv_smem + (uint32_t)(s * kStageBytesT + kv * 2 * kTile16K + half * 8192);
+            ptx::tma_load_2d(dst, &tm_kv, c0, row, full_bar(s), ptx::kEvictLast);
+            ptx::tma_load_2d(dst + kTile16K, &tm_kv, c0 + 64, row, full_bar(s), ptx::kEvictLast);
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===== consumers: warpgroup g owns tile rows [64 g, 64 g + 64); this thread rows mr[0], mr[1] =====
+  const int g = warp >> 2;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  int mr[2], qpos[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    mr[h] = g * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    qpos[h] = pos_first + mr[h] / p.R;
+  }
+  const int cq = 2 * (lane & 3);                         // first of this thread's two columns in each 8-column group
+  float o[64];
+#pragma unroll
+  for (int e = 0; e < 64; ++e) o[e] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // m_run: the exponent P and l are relative to
+
+  ptx::mbar_wait(q_bar, 0);
+  for (int i = 0; i < n_it; ++i) {
+    const int s = i % kStagesT;
+    ptx::mbar_wait(full_bar(s), (uint32_t)((i / kStagesT) & 1));
+    const uint32_t k_addr = kv_smem + (uint32_t)(s * kStageBytesT);
+    const uint32_t v_addr = k_addr + 2 * kTile16K;
+    float sv[64];
+    ptx::wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      const uint64_t a = ptx::make_kmajor_sw128_desc(q_smem + (uint32_t)((ks >> 2) * kTile16K + g * 8192)) + (uint64_t)(2 * (ks & 3));
+      const uint64_t b = ptx::make_kmajor_sw128_desc(k_addr + (uint32_t)((ks >> 2) * kTile16K)) + (uint64_t)(2 * (ks & 3));
+      ptx::wgmma_ss<0, 0>(sv, a, b, ks > 0 ? 1u : 0u);
+    }
+    ptx::wg_commit();
+    ptx::wg_wait<0>();
+    ptx::fence_acc(sv);
+    const int key0 = i * kKeys;
+    if (key0 + kKeys - 1 > pos_first) {                  // some (row, key) of this step is causally masked
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (key0 + 8 * j + cq + (e & 1) > qpos[e >> 1]) sv[4 * j + e] = -INFINITY;
+    }
+    float alpha[2], m_use[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) mx = fmaxf(mx, fmaxf(sv[4 * j + 2 * h], sv[4 * j + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx * p.scale_log2);   // scale > 0: max commutes with the scaling
+      if (!kLazyRescale || m_new > m_run[h] + 8.f) {
+        m_use[h] = (m_new == -INFINITY) ? 0.f : m_new;
+        alpha[h] = ex2(m_run[h] - m_use[h]);              // 0 on the first step
+        m_run[h] = m_new;
+      } else {                                            // keep the reference: P <= 2^8
+        m_use[h] = (m_run[h] == -INFINITY) ? 0.f : m_run[h];
+        alpha[h] = 1.f;
+      }
+    }
+    if (!kLazyRescale || alpha[0] != 1.f || alpha[1] != 1.f) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        o[4 * j] *= alpha[0]; o[4 * j + 1] *= alpha[0];
+        o[4 * j + 2] *= alpha[1]; o[4 * j + 3] *= alpha[1];
+      }
+    }
+    float sum[2] = {0.f, 0.f};
+    uint32_t pa[8][4];                                   // P as the A fragments of the 8 k16 steps of P V
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const float p0 = ex2(fmaf(sv[4 * j], p.scale_log2, -m_use[0]));       // masked entries: exp2(-inf) = 0
+      const float p1 = ex2(fmaf(sv[4 * j + 1], p.scale_log2, -m_use[0]));
+      const float p2 = ex2(fmaf(sv[4 * j + 2], p.scale_log2, -m_use[1]));
+      const float p3 = ex2(fmaf(sv[4 * j + 3], p.scale_log2, -m_use[1]));
+      sum[0] += p0 + p1;
+      sum[1] += p2 + p3;
+      pa[j >> 1][(j & 1) * 2] = pack2(p0, p1);
+      pa[j >> 1][(j & 1) * 2 + 1] = pack2(p2, p3);
+    }
+    l_run[0] = l_run[0] * alpha[0] + sum[0];             // this thread's share of the row sums
+    l_run[1] = l_run[1] * alpha[1] + sum[1];
+    ptx::fence_acc(o);
+    ptx::wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)
+      ptx::wgmma_rs<1>(o, pa[kk], ptx::make_mnmajor_sw128_desc(v_addr, kTile16K) + (uint64_t)(128 * kk), 1u);
+    ptx::wg_commit();
+    ptx::wg_wait<0>();
+    ptx::fence_acc(o);
+    if (wg_leader) ptx::mbar_arrive(empty_bar(s));       // K and V of this stage are consumed
+  }
+
+  // ---- epilogue: normalise, write bf16 rows (and the log2-domain log-sum-exp the backward needs) ----
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const int qi = mr[h] / p.R, r = mr[h] - qi * p.R;
+    if (qi >= n_valid) continue;
+    const float inv = l > 0.f ? 1.f / l : 0.f;
+    if (kContig && p.lse != nullptr && (lane & 3) == 0)  // P = exp2(s * scale_log2 - lse) in the backward
+      p.lse[(int64_t)(row0 + qi) * p.n_q + (kvh * p.R + r)] = m_run[h] + log2f(l);
+    __nv_bfloat16* dst = p.out + ((int64_t)(row0 + qi) * p.n_q + (kvh * p.R + r)) * kDT + cq;
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+      *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack2(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
+  }
 }
 
 template <bool kContig>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreadsT, 1)
-attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_kv,
-                       TcPrefillParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t q_smem = base;                          // Q lo | Q hi
-  const uint32_t kv_smem = base + 2 * kTile16K;          // 2 stages x (K lo | K hi | V lo | V hi)
-  const uint32_t p_smem = kv_smem + 2 * kStageBytesT;    // 2 buffers x (P keys 0..63 | keys 64..127)
-  const uint32_t bar_base = p_smem + 4 * kTile16K;
-  auto bar = [&](int i) { return bar_base + 8u * (uint32_t)i; };
-  // 0 q_full | 1,2 k_full | 3,4 k_empty | 5,6 s_full | 7,8 s_empty | 9,14 p_full | 10,11 o_full | 12,13 o_empty |
-  // 15,16 v_full | 17,18 v_empty.   K and V slots cycle independently: a K slot is free as soon as its Q K^T has run,
-  // so K of step i+2 streams in during the softmax of step i and S is always ready when the softmax warps want it.
-  const uint32_t tmem_slot = bar(19);
-
-  // The two CTAs of a cluster own ADJACENT query tiles of the same (sequence, kv head): they walk the same K/V pages,
-  // so each CTA fetches one of the two pages of a step and TMA-multicasts it into both CTAs' shared memory -- the
-  // kernel is bound by L2 -> SM bandwidth (64 KB of K/V per 8.4 MFLOP step and CTA), and this halves it.
-  // packed training rows are long and causal: walk the query tiles heaviest-first (adjacent tiles stay a cluster pair)
-  const int qtile = kContig ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
-  const int kvh = blockIdx.y, z = blockIdx.z;
-  const uint32_t rank = ptx::cluster_ctarank();
-  const int q_len = ptx::warp_uniform(p.seq_q_len[z]);
-  const int pos0 = kContig ? 0 : ptx::warp_uniform(p.seq_pos0[z]);
-  if ((qtile & ~1) * p.nq >= q_len) return;              // uniform across the CLUSTER, before any barrier / TMEM use
-  const int t0 = qtile * p.nq;
-  const int row0 = ptx::warp_uniform(p.seq_q_start[z]) + t0;
-  const int pos_first = pos0 + t0;
-  const int n_valid = t0 >= q_len ? 0 : ((q_len - t0) < p.nq ? (q_len - t0) : p.nq);  // 0: partner-only CTA
-  // both CTAs run the step count of the LATER tile (the earlier tile's extra step is fully masked)
-  const int pair_rows = ((qtile | 1) + 1) * p.nq;
-  const int kv_end = pos0 + (pair_rows < q_len ? pair_rows : q_len);
-  const int n_it = (kv_end + kKeys - 1) / kKeys;
-  const int last_page = (kv_end - 1) / kPageT;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 19; ++i) ptx::mbar_init(bar(i), (i == 3 || i == 4 || i == 17 || i == 18) ? 2 : 1);  // *_empty: both CTAs' MMA warps
-    ptx::fence_barrier_init();
-    ptx::fence_proxy_async();
-    ptx::prefetch_tensormap(&tm_q);
-    ptx::prefetch_tensormap(&tm_kv);
-  }
-  if (warp == 1) {
-    ptx::tmem_alloc(tmem_slot, 512);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before_sync();
-  ptx::cluster_sync();                                   // the partner's barriers exist before anything targets them
-  ptx::tc_fence_after_sync();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-  tmem_base = ptx::warp_uniform(tmem_base);
-
-  if (warp == 0) {
-    // ===== TMA producer =====
-    if (lane == 0) {
-      ptx::mbar_arrive_expect_tx(bar(0), (uint32_t)(2 * 128 * p.R * p.nq));
-      ptx::tma_load_3d(q_smem, &tm_q, 0, kvh * p.R, row0, bar(0), ptx::kEvictFirst);
-      ptx::tma_load_3d(q_smem + kTile16K, &tm_q, 64, kvh * p.R, row0, bar(0), ptx::kEvictFirst);
-      const int32_t* bt = kContig ? nullptr : p.block_table + (int64_t)p.seq_slot[z] * p.max_blocks;
-      const int seq_row0 = p.seq_q_start[z];
-      // this CTA fetches ONE of the two pages of a step (rank 0: keys 0..63, rank 1: keys 64..127) and multicasts it
-      auto load_page = [&](int it, int kv, uint32_t full_bar, uint32_t empty_bar) {
-        const int s = it & 1;
-        const uint32_t ph = (uint32_t)((it >> 1) & 1);
-        ptx::mbar_wait(empty_bar + 8u * (uint32_t)s, ph ^ 1u);
-        ptx::mbar_arrive_expect_tx(full_bar + 8u * (uint32_t)s, (uint32_t)(2 * kTile16K));
-        int pg = 2 * it + (int)rank;
-        if (pg > last_page) pg = last_page;              // the tail step re-reads the last page; its keys are masked
-        int row, c0;
-        if (kContig) {                                   // rows past the sequence / past T: masked keys (TMA zero-fills OOB)
-          row = seq_row0 + pg * kPageT;
-          c0 = (kv ? p.col_v : p.col_k) + kvh * kDT;
-        } else {
-          const int page = bt[pg];
-          row = (int)(((((int64_t)p.layer * 2 + kv) * p.n_pages + page) * p.n_kv + kvh) * kPageT);
-          c0 = 0;
-        }
-        const uint32_t dst = kv_smem + (uint32_t)(s * kStageBytesT + kv * 2 * kTile16K) + (uint32_t)(rank * 8192);
-        ptx::tma_load_2d_multicast(dst, &tm_kv, c0, row, full_bar + 8u * (uint32_t)s, 3, ptx::kEvictLast);
-        ptx::tma_load_2d_multicast(dst + kTile16K, &tm_kv, c0 + 64, row, full_bar + 8u * (uint32_t)s, 3, ptx::kEvictLast);
-      };
-      load_page(0, 0, bar(1), bar(3));
-      for (int it = 0; it < n_it; ++it) {                // same order as the MMA warp consumes: K(it+1), then V(it)
-        if (it + 1 < n_it) load_page(it + 1, 0, bar(1), bar(3));
-        load_page(it, 1, bar(15), bar(17));
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    {   // the whole warp, converged: one elected lane issues each tcgen05 instruction (ptx::elect_one)
-      constexpr uint32_t idesc_qk = ptx::make_idesc_bf16_f32(128, kKeys);
-      constexpr uint32_t idesc_pv = ptx::make_idesc_bf16_f32(128, kDT) | (1u << 16);  // B (= V) is MN-major
-      auto issue_qk = [&](int j) {
-        const int s = j & 1;
-        const uint32_t ph = (uint32_t)((j >> 1) & 1);
-        ptx::mbar_wait(bar(1 + s), ph);          // K of step j landed
-        ptx::mbar_wait(bar(7 + s), ph ^ 1u);     // S[s] drained by the softmax warps (step j - 2)
-        ptx::tc_fence_after_sync();
-        const uint32_t k_addr = kv_smem + (uint32_t)(s * kStageBytesT);
-        if (ptx::elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {
-            const uint64_t a = ptx::make_kmajor_sw128_desc(q_smem + (uint32_t)((ks >> 2) * kTile16K)) + (uint64_t)(2 * (ks & 3));
-            const uint64_t b = ptx::make_kmajor_sw128_desc(k_addr + (uint32_t)((ks >> 2) * kTile16K)) + (uint64_t)(2 * (ks & 3));
-            ptx::mma_bf16_ss(tmem_base + (uint32_t)(s * 128), a, b, idesc_qk, ks > 0 ? 1u : 0u);
-          }
-          ptx::tc_commit(bar(5 + s));
-          ptx::tc_commit_multicast(bar(3 + s), 3);  // K slot consumed here: tell BOTH producers
-        }
-      };
-      ptx::mbar_wait(bar(0), 0);
-      issue_qk(0);
-      for (int i = 0; i < n_it; ++i) {
-        if (i + 1 < n_it) issue_qk(i + 1);
-        const int s = i & 1;
-        const uint32_t ph = (uint32_t)((i >> 1) & 1);
-        ptx::mbar_wait(bar(s ? 14 : 9), ph);         // P[s] of step i is in shared memory
-        ptx::mbar_wait(bar(12 + s), ph ^ 1u);        // Ot[s] folded by the softmax warps (step i - 2)
-        ptx::mbar_wait(bar(15 + s), ph);             // V of step i landed
-        ptx::tc_fence_after_sync();
-        const uint32_t v_addr = kv_smem + (uint32_t)(s * kStageBytesT) + 2 * kTile16K;
-        const uint32_t p_addr = p_smem + (uint32_t)(s * 2 * kTile16K);
-        if (ptx::elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {
-            const uint64_t a = ptx::make_kmajor_sw128_desc(p_addr + (uint32_t)((ks >> 2) * kTile16K)) + (uint64_t)(2 * (ks & 3));
-            const uint64_t b = ptx::make_mnmajor_sw128_desc(v_addr, kTile16K) + (uint64_t)(128 * ks);
-            ptx::mma_bf16_ss(tmem_base + (uint32_t)(256 + s * 128), a, b, idesc_pv, ks > 0 ? 1u : 0u);
-          }
-          ptx::tc_commit(bar(10 + s));   // Ot[s] complete (and P[s] free again)
-          ptx::tc_commit_multicast(bar(17 + s), 3);  // V slot consumed here: tell BOTH producers
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===== softmax + epilogue: 8 warps; a PAIR of threads owns one (token, head) row =====
-    // warp w may only touch TMEM lanes 32 (w % 4) ..; the two warps of a lane quarter split the row: half h works on
-    // keys [64 h, 64 h + 64) of every step (S kept in registers: one TMEM read) and on head-dim columns
-    // [64 h, 64 h + 64) of the output accumulator.  The row maximum is exchanged through shared memory.
-    const int q = warp & 3;
-    const int h = (warp - 2) >> 2;
-    const int m = q * 32 + lane;
-    const int qi = m / p.R, r = m - qi * p.R;
-    const int qpos = pos_first + qi;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    const uint32_t p_row0 = p_smem + (uint32_t)(h * kTile16K + m * 128);
-    float* xchg = reinterpret_cast<float*>(smem_raw + (bar_base - ptx::smem_u32(smem_raw)) + 8 * 20);  // [2][128]
-    float m_run = -INFINITY, l_run = 0.f, alpha_prev = 0.f;
-    float o[64];
-#pragma unroll
-    for (int d = 0; d < 64; ++d) o[d] = 0.f;
-
-    auto fold = [&](int j) {   // o = o * alpha_j + Ot_j   (this thread's 64 head-dim columns)
-      const int s = j & 1;
-      ptx::mbar_wait(bar(10 + s), (uint32_t)((j >> 1) & 1));
-      ptx::tc_fence_after_sync();
-      uint32_t v0[32], v1[32];
-      ptx::tmem_ld_32x32b_x32(lane_addr + (uint32_t)(256 + s * 128 + h * 64), v0);
-      ptx::tmem_ld_32x32b_x32(lane_addr + (uint32_t)(256 + s * 128 + h * 64 + 32), v1);
-      ptx::tmem_ld_wait();
-#pragma unroll
-      for (int e = 0; e < 32; ++e) {
-        o[e] = fmaf(o[e], alpha_prev, __uint_as_float(v0[e]));
-        o[32 + e] = fmaf(o[32 + e], alpha_prev, __uint_as_float(v1[e]));
-      }
-      ptx::tc_fence_before_sync();
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (threadIdx.x == 64) ptx::mbar_arrive(bar(12 + s));
-    };
-
-    for (int i = 0; i < n_it; ++i) {
-      const int s = i & 1;
-      ptx::mbar_wait(bar(5 + s), (uint32_t)((i >> 1) & 1));
-      ptx::tc_fence_after_sync();
-      const int key0 = i * kKeys + h * 64;
-      const bool diag = i * kKeys + kKeys - 1 > pos_first;   // some (row, key) of this step is masked
-      float sv[64];
-      {
-        uint32_t v0[32], v1[32];
-        ptx::tmem_ld_32x32b_x32(lane_addr + (uint32_t)(s * 128 + h * 64), v0);
-        ptx::tmem_ld_32x32b_x32(lane_addr + (uint32_t)(s * 128 + h * 64 + 32), v1);
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int e = 0; e < 32; ++e) { sv[e] = __uint_as_float(v0[e]); sv[32 + e] = __uint_as_float(v1[e]); }
-      }
-      if (diag) {
-#pragma unroll
-        for (int e = 0; e < 64; ++e)
-          if (key0 + e > qpos) sv[e] = -INFINITY;
-      }
-      float mx = -INFINITY;
-#pragma unroll
-      for (int e = 0; e < 64; ++e) mx = fmaxf(mx, sv[e]);
-      xchg[h * 128 + m] = mx;
-      ptx::tc_fence_before_sync();
-      asm volatile("bar.sync 1, 256;" ::: "memory");       // S[s] is in registers on every thread; maxima exchanged
-      if (threadIdx.x == 64) ptx::mbar_arrive(bar(7 + s));  // S[s] drained -> Q K^T of step i + 2 may overwrite it
-      mx = fmaxf(mx, xchg[(1 - h) * 128 + m]) * p.scale_log2;  // scale > 0: max commutes with the scaling
-      const float m_new = fmaxf(m_run, mx);
-      const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-      const float alpha = ex2(m_run - m_use);               // 0 on the first step
-      // P[s] is free: P V of step i - 2 completed before fold(i - 2) returned during step i - 1
-      const uint32_t p_row = p_row0 + (uint32_t)(s * 2 * kTile16K);
-      float sum = 0.f;
-#pragma unroll
-      for (int j = 0; j < 64; j += 8) {
-        float pe[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          pe[e] = ex2(fmaf(sv[j + e], p.scale_log2, -m_use));   // masked entries: exp2(-inf) = 0
-          sum += pe[e];
-        }
-        st_shared_v4(p_row + (((uint32_t)(j >> 3) ^ (uint32_t)(m & 7)) << 4), pack2(pe[0], pe[1]), pack2(pe[2], pe[3]),
-                     pack2(pe[4], pe[5]), pack2(pe[6], pe[7]));
-      }
-      l_run = l_run * alpha + sum;                           // this half's share of the row sum
-      m_run = m_new;
-      ptx::fence_proxy_async();                              // generic-proxy stores of P -> visible to the UMMA reads
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (threadIdx.x == 64) ptx::mbar_arrive(bar(s ? 14 : 9));   // P[s] ready -> P V of step i starts
-      // fold the PREVIOUS step while the tensor core runs this step's P V (its own P V finished during the exp phase)
-      if (i > 0) fold(i - 1);
-      alpha_prev = alpha;
-    }
-    fold(n_it - 1);
-    xchg[h * 128 + m] = l_run;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    const float l_tot = l_run + xchg[(1 - h) * 128 + m];
-    if (qi < n_valid && qi < p.nq) {
-      const float inv = l_tot > 0.f ? 1.f / l_tot : 0.f;
-      if (kContig && p.lse != nullptr && h == 0)          // P = exp2(s * scale_log2 - lse) in the backward
-        p.lse[(int64_t)(row0 + qi) * p.n_q + (kvh * p.R + r)] = m_run + log2f(l_tot);
-      __nv_bfloat16* dst = p.out + ((int64_t)(row0 + qi) * p.n_q + (kvh * p.R + r)) * kDT + h * 64;
-#pragma unroll
-      for (int d = 0; d < 64; d += 8) {
-        uint4 u;
-        u.x = pack2(o[d] * inv, o[d + 1] * inv);
-        u.y = pack2(o[d + 2] * inv, o[d + 3] * inv);
-        u.z = pack2(o[d + 4] * inv, o[d + 5] * inv);
-        u.w = pack2(o[d + 6] * inv, o[d + 7] * inv);
-        *reinterpret_cast<uint4*>(dst + d) = u;
-      }
-    }
-  }
-
-  ptx::tc_fence_before_sync();
-  ptx::cluster_sync();   // the partner may still multicast into this CTA's shared memory / arrive on its barriers
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc(tmem_base, 512);
-  }
+cudaError_t launch_fwd(int generation, dim3 grid, const CUtensorMap& tq, const CUtensorMap& tkv, const TcPrefillParams& p,
+                       cudaStream_t stream) {
+  static SmemAttr smem_attr[2] = {};
+  auto kernel = generation == 1 ? attn_fwd_kernel<kContig, false> : attn_fwd_kernel<kContig, true>;
+  cudaError_t e = ensure_smem(kernel, kSmemT, smem_attr[generation == 1 ? 0 : 1]);
+  if (e != cudaSuccess) return e;
+  kernel<<<grid, kThreadsT, (size_t)kSmemT, stream>>>(tq, tkv, p);
+  return cudaSuccess;
 }
 
-
-// =====================================================================================================
-// Forward, second generation: two softmax groups in ping-pong, O accumulated in TMEM.
-//
-// The first-generation kernel above runs its eight softmax warps in lock-step through  load S -> max -> exp -> store P ->
-// fold O:  the MUFU pipe and the tensor pipe take turns instead of overlapping, and the softmax warps' instruction stream
-// (not the tensor pipe, not TMEM, not shared memory: profiles/r2_attention.md) is what a step waits for.  Here:
-//   * softmax group g (4 warps, ONE THREAD PER ROW, all 128 keys of a step in registers) owns the steps i = g (mod 2)
-//     with its own online-softmax state (reference exponent m_ref, row sum l) and its own accumulator O_g in TMEM:
-//     while group 0 exponentiates step i, group 1 loads / maximises / stores step i + 1 and the tensor core runs the
-//     Q K^T of step i + 2 and the P V of step i - 1.  The two partial results are merged once, at the end
-//     (a log-sum-exp merge, as for split-KV decode).
-//   * P_g is handed to the tensor core THROUGH TMEM (tcgen05.mma with the A operand in tensor memory), written by each
-//     thread into its own row in place of the S values it has just consumed: no shared-memory store, no proxy fence, no
-//     A-operand fetch from shared memory, and the 64 KB generation 1 spends on P buffers become a third K/V stage.
-//   * O_g is NEVER read inside the loop: P V accumulates into it (tcgen05.mma accumulate), and a row is rescaled in TMEM
-//     (tcgen05.ld / scale / tcgen05.st) only when its running maximum grew by more than 2^8 since the reference was
-//     set -- P stays below 256, exact in bf16's range, and for trained or random scores the rescale branch is taken in
-//     the first steps of a row only.
-// TMEM: S_0 | S_1 | O_0 | O_1 (4 x 128 columns).  Shared memory and the K/V cluster multicast are those of generation 1.
-// =====================================================================================================
-__device__ __forceinline__ void group_bar(int g) {
-  if (g == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
-  else asm volatile("bar.sync 2, 128;" ::: "memory");
-}
-
-template <bool kContig, bool kTimed = false>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreadsT, 1)   // 10 warps: 3 share one SMSP -> 168 registers
-attn_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_kv, TcPrefillParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t q_smem = base;                          // Q lo | Q hi
-  const uint32_t kv_smem = base + 2 * kTile16K;          // 3 stages x (K lo | K hi | V lo | V hi): P lives in TMEM, so the
-  //                                                        64 KB generation 1 spends on P buffers buy a third K/V stage --
-  //                                                        K / V of step i + 2 are requested as soon as step i - 1 is done
-  constexpr int kSt = 3;
-  const uint32_t bar_base = kv_smem + kSt * kStageBytesT;
-  auto bar = [&](int i) { return bar_base + 8u * (uint32_t)i; };
-  // 0 q_full | 1..3 k_full | 4..6 k_empty | 7,8 s_full | 9,10 p_full | 11,12 o_full | 13..15 v_full | 16..18 v_empty
-  const uint32_t tmem_slot = bar(19);
-
-  const int qtile = kContig ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
-  const int kvh = blockIdx.y, z = blockIdx.z;
-  const uint32_t rank = ptx::cluster_ctarank();
-  const int q_len = ptx::warp_uniform(p.seq_q_len[z]);
-  const int pos0 = (kContig && p.seq_pos0 == nullptr) ? 0 : ptx::warp_uniform(p.seq_pos0[z]);
-  if ((qtile & ~1) * p.nq >= q_len) return;              // uniform across the CLUSTER, before any barrier / TMEM use
-  const int t0 = qtile * p.nq;
-  const int row0 = ptx::warp_uniform(p.seq_q_start[z]) + t0;
-  const int pos_first = pos0 + t0;
-  const int n_valid = t0 >= q_len ? 0 : ((q_len - t0) < p.nq ? (q_len - t0) : p.nq);
-  const int pair_rows = ((qtile | 1) + 1) * p.nq;
-  const int kv_end = pos0 + (pair_rows < q_len ? pair_rows : q_len);
-  const int n_it = (kv_end + kKeys - 1) / kKeys;
-  const int last_page = (kv_end - 1) / kPageT;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 19; ++i) ptx::mbar_init(bar(i), ((i >= 4 && i <= 6) || (i >= 16 && i <= 18)) ? 2 : 1);   // *_empty: both CTAs
-    ptx::fence_barrier_init();
-    ptx::fence_proxy_async();
-    ptx::prefetch_tensormap(&tm_q);
-    ptx::prefetch_tensormap(&tm_kv);
-  }
-  if (warp == 1) {
-    ptx::tmem_alloc(tmem_slot, 512);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before_sync();
-  ptx::cluster_sync();
-  ptx::tc_fence_after_sync();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-  tmem_base = ptx::warp_uniform(tmem_base);
-
-  if (warp == 0) {
-    // ===== TMA producer (as generation 1) =====
-    if (lane == 0) {
-      ptx::mbar_arrive_expect_tx(bar(0), (uint32_t)(2 * 128 * p.R * p.nq));
-      ptx::tma_load_3d(q_smem, &tm_q, 0, kvh * p.R, row0, bar(0), ptx::kEvictFirst);
-      ptx::tma_load_3d(q_smem + kTile16K, &tm_q, 64, kvh * p.R, row0, bar(0), ptx::kEvictFirst);
-      const int32_t* bt = kContig ? nullptr : p.block_table + (int64_t)p.seq_slot[z] * p.max_blocks;
-      const int seq_row0 = (kContig && p.seq_kv_start != nullptr) ? p.seq_kv_start[z] : p.seq_q_start[z];
-      auto load_page = [&](int it, int kv, uint32_t full_bar, uint32_t empty_bar) {
-        const int s = it % kSt;
-        const uint32_t ph = (uint32_t)((it / kSt) & 1);
-        ptx::mbar_wait(empty_bar + 8u * (uint32_t)s, ph ^ 1u);
-        ptx::mbar_arrive_expect_tx(full_bar + 8u * (uint32_t)s, (uint32_t)(2 * kTile16K));
-        int pg = 2 * it + (int)rank;
-        if (pg > last_page) pg = last_page;
-        int row, c0;
-        if (kContig) {
-          row = seq_row0 + pg * kPageT;
-          c0 = (kv ? p.col_v : p.col_k) + kvh * kDT;
-        } else {
-          const int page = bt[pg];
-          row = (int)(((((int64_t)p.layer * 2 + kv) * p.n_pages + page) * p.n_kv + kvh) * kPageT);
-          c0 = 0;
-        }
-        const uint32_t dst = kv_smem + (uint32_t)(s * kStageBytesT + kv * 2 * kTile16K) + (uint32_t)(rank * 8192);
-        ptx::tma_load_2d_multicast(dst, &tm_kv, c0, row, full_bar + 8u * (uint32_t)s, 3, ptx::kEvictLast);
-        ptx::tma_load_2d_multicast(dst + kTile16K, &tm_kv, c0 + 64, row, full_bar + 8u * (uint32_t)s, 3, ptx::kEvictLast);
-      };
-      load_page(0, 0, bar(1), bar(4));
-      for (int it = 0; it < n_it; ++it) {
-        if (it + 1 < n_it) load_page(it + 1, 0, bar(1), bar(4));
-        load_page(it, 1, bar(13), bar(16));
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    {   // the whole warp, converged: one elected lane issues each tcgen05 instruction (ptx::elect_one)
-      constexpr uint32_t idesc_qk = ptx::make_idesc_bf16_f32(128, kKeys);
-      constexpr uint32_t idesc_pv = ptx::make_idesc_bf16_f32(128, kDT) | (1u << 16);  // B (= V) is MN-major
-      auto issue_qk = [&](int j) {
-        const int s = j & 1;                     // S buffer / softmax group
-        const int ks_ = j % kSt;                 // K/V stage
-        ptx::mbar_wait(bar(1 + ks_), (uint32_t)((j / kSt) & 1));   // K of step j landed
-        // S_s's columns held P_s of step j - 2: its P V was issued before this point and UMMAs of one thread execute in
-        // issue order, so this Q K^T cannot overtake it (and the softmax group finished reading S_s before it stored P_s)
-        ptx::tc_fence_after_sync();
-        const uint32_t k_addr = kv_smem + (uint32_t)(ks_ * kStageBytesT);
-        if (ptx::elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {
-            const uint64_t a = ptx::make_kmajor_sw128_desc(q_smem + (uint32_t)((ks >> 2) * kTile16K)) + (uint64_t)(2 * (ks & 3));
-            const uint64_t b = ptx::make_kmajor_sw128_desc(k_addr + (uint32_t)((ks >> 2) * kTile16K)) + (uint64_t)(2 * (ks & 3));
-            ptx::mma_bf16_ss(tmem_base + (uint32_t)(s * 128), a, b, idesc_qk, ks > 0 ? 1u : 0u);
-          }
-          ptx::tc_commit(bar(7 + s));
-          ptx::tc_commit_multicast(bar(4 + ks_), 3);
-        }
-      };
-      const bool timed = kTimed && p.timing != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
-      long long w_p = 0, w_v = 0, w_tot0 = clock64();
-      ptx::mbar_wait(bar(0), 0);
-      issue_qk(0);
-      for (int i = 0; i < n_it; ++i) {
-        if (i + 1 < n_it) issue_qk(i + 1);
-        const int s = i & 1;
-        const uint32_t ph = (uint32_t)((i >> 1) & 1);
-        const int vs_ = i % kSt;
-        const long long c0 = clock64();
-        ptx::mbar_wait(bar(9 + s), ph);              // P_s of step i is in TMEM (and O_s rescaled if it had to be)
-        const long long c1 = clock64();
-        ptx::mbar_wait(bar(13 + vs_), (uint32_t)((i / kSt) & 1));   // V of step i landed
-        if (kTimed) { w_p += c1 - c0; w_v += clock64() - c1; }
-        ptx::tc_fence_after_sync();
-        const uint32_t v_addr = kv_smem + (uint32_t)(vs_ * kStageBytesT) + 2 * kTile16K;
-        if (ptx::elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {             // A = P_s out of TMEM: 16 keys = 8 packed columns per UMMA
-            const uint64_t b = ptx::make_mnmajor_sw128_desc(v_addr, kTile16K) + (uint64_t)(128 * ks);
-            ptx::mma_bf16_ts(tmem_base + (uint32_t)(256 + s * 128), tmem_base + (uint32_t)(s * 128 + ks * 8), b, idesc_pv,
-                             (i >= 2 || ks > 0) ? 1u : 0u);
-          }
-          ptx::tc_commit(bar(11 + s));                 // O_s updated
-          ptx::tc_commit_multicast(bar(16 + vs_), 3);  // V slot consumed: tell BOTH producers
-        }
-      }
-      if (timed && lane == 0) { p.timing[16] = w_p; p.timing[17] = w_v; p.timing[18] = clock64() - w_tot0; p.timing[19] = n_it; }
-    }
-    __syncwarp();
-  } else {
-    // ===== softmax: group g = steps i = g (mod 2); one thread per (token, head) row =====
-    const int g = (warp - 2) >> 2;
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int qi = m / p.R, r = m - qi * p.R;
-    const int qpos = pos_first + qi;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    const uint32_t s_addr = lane_addr + (uint32_t)(g * 128);
-    const uint32_t o_addr = lane_addr + (uint32_t)(256 + g * 128);
-    const bool leader = (threadIdx.x == 64 + g * 128);
-    float2* xchg = reinterpret_cast<float2*>(smem_raw + (bar_base - ptx::smem_u32(smem_raw)) + 8 * 20);  // [128] (m_ref, l) of group 1
-    float m_ref = 0.f, l_run = 0.f;
-    const bool timed = kTimed && p.timing != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && q == 0 && lane == 0;
-    long long tph[6] = {0, 0, 0, 0, 0, 0};
-
-    for (int i = g; i < n_it; i += 2) {
-      const int j = i >> 1;
-      const long long c0 = clock64();
-      ptx::mbar_wait(bar(7 + g), (uint32_t)(j & 1));
-      ptx::tc_fence_after_sync();
-      const long long c1 = clock64();
-      float sv[128];
-      {
-        uint32_t su[128];                                   // four 32-column reads in flight, one wait
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          ptx::tmem_ld_32x32b_x32(s_addr + (uint32_t)(c * 32), *reinterpret_cast<uint32_t(*)[32]>(&su[c * 32]));
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int e = 0; e < 128; ++e) sv[e] = __uint_as_float(su[e]);
-      }
-      const long long c2 = clock64();
-      if (i * kKeys + kKeys - 1 > pos_first) {              // some (row, key) of this step is causally masked
-        const int key0 = i * kKeys;
-#pragma unroll
-        for (int e = 0; e < 128; ++e)
-          if (key0 + e > qpos) sv[e] = -INFINITY;
-      }
-      float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};   // four independent chains of 3-input maxima (FMNMX3):
-#pragma unroll                                                       // 64 instructions for the 128 scores of a row
-      for (int e = 0; e < 128; e += 8) {
-        mx4[0] = max3(mx4[0], sv[e], sv[e + 1]); mx4[1] = max3(mx4[1], sv[e + 2], sv[e + 3]);
-        mx4[2] = max3(mx4[2], sv[e + 4], sv[e + 5]); mx4[3] = max3(mx4[3], sv[e + 6], sv[e + 7]);
-      }
-      const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-      const float m_new = mx * p.scale_log2;                // scale > 0: max commutes with the scaling
-      const long long c3 = clock64();
-      if (j == 0) {
-        m_ref = (m_new == -INFINITY) ? 0.f : m_new;
-      } else {
-        const bool need = m_new > m_ref + 8.f;              // rows of a warp decide together (TMEM ops are warp-wide)
-        if (__any_sync(0xffffffffu, need)) {
-          // O_g is touched only here: wait for P V of step i - 2.  Skipping the wait on the other steps is safe -- phase j of
-          // this barrier needs P of own step j, which this thread has not produced yet, so at own step j the barrier is
-          // either still in phase j - 1 or has just completed it: the parity test cannot alias an older phase.
-          ptx::mbar_wait(bar(11 + g), (uint32_t)((j - 1) & 1));
-          ptx::tc_fence_after_sync();
-          const float f = need ? ex2(m_ref - m_new) : 1.f;
-#pragma unroll 1
-          for (int c = 0; c < 8; ++c) {                     // rare path: small chunks keep the S row in registers
-            uint32_t v[16];
-            ptx::tmem_ld_32x32b_x16(o_addr + (uint32_t)(c * 16), v);
-            ptx::tmem_ld_wait();
-#pragma unroll
-            for (int e = 0; e < 16; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) * f);
-            ptx::tmem_st_32x32b_x16(o_addr + (uint32_t)(c * 16), v);
-          }
-          ptx::tmem_st_wait();
-          l_run *= f;
-          if (need) m_ref = m_new;
-        }
-      }
-      // P_g goes back into TMEM as the A operand of P V, in place of this row's own S values (lane = row; one 32-bit column
-      // = two adjacent keys): no shared-memory store, no shared-memory read by the tensor core
-      const long long c4 = clock64();
-      float sum4[4] = {0.f, 0.f, 0.f, 0.f};                 // independent partial row sums (fixed order: deterministic)
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t pp[16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const float p0 = ex2(fmaf(sv[c * 32 + 2 * e], p.scale_log2, -m_ref));       // masked entries: exp2(-inf) = 0
-          const float p1 = ex2(fmaf(sv[c * 32 + 2 * e + 1], p.scale_log2, -m_ref));
-          sum4[e & 3] += p0 + p1;
-          pp[e] = pack2(p0, p1);
-        }
-        ptx::tmem_st_32x32b_x16(s_addr + (uint32_t)(c * 16), pp);
-      }
-      l_run += (sum4[0] + sum4[1]) + (sum4[2] + sum4[3]);
-      ptx::tmem_st_wait();
-      const long long c5 = clock64();
-      ptx::tc_fence_before_sync();
-      group_bar(g);
-      if (leader) ptx::mbar_arrive(bar(9 + g));             // P_g ready -> P V of step i
-      if (timed) {
-        const long long c6 = clock64();
-        tph[0] += c1 - c0; tph[1] += c2 - c1; tph[2] += c3 - c2; tph[3] += c4 - c3; tph[4] += c5 - c4; tph[5] += c6 - c5;
-      }
-    }
-    if (timed) {
-#pragma unroll
-      for (int e = 0; e < 6; ++e) p.timing[g * 8 + e] = tph[e];
-    }
-
-    // ---- merge the two groups' partial results and write the output rows (group 0) ----
-    const int n1 = n_it >> 1;                               // steps of group 1
-    if (g == 1) xchg[m] = make_float2(m_ref, l_run);
-    asm volatile("bar.sync 3, 256;" ::: "memory");
-    if (g == 0) {
-      const int n0 = (n_it + 1) >> 1;
-      ptx::mbar_wait(bar(11), (uint32_t)((n0 - 1) & 1));
-      if (n1 > 0) ptx::mbar_wait(bar(12), (uint32_t)((n1 - 1) & 1));
-      ptx::tc_fence_after_sync();
-      float m1 = 0.f, l1 = 0.f;
-      if (n1 > 0) { const float2 x = xchg[m]; m1 = x.x; l1 = x.y; }
-      const bool use1 = n1 > 0 && l1 > 0.f;
-      const bool use0 = l_run > 0.f;
-      const float m_all = use0 ? (use1 ? fmaxf(m_ref, m1) : m_ref) : m1;
-      const float f0 = use0 ? ex2(m_ref - m_all) : 0.f;
-      const float f1 = use1 ? ex2(m1 - m_all) : 0.f;
-      const float l_tot = f0 * l_run + f1 * l1;
-      const float inv = l_tot > 0.f ? 1.f / l_tot : 0.f;
-      const bool valid = qi < n_valid && qi < p.nq;
-      __nv_bfloat16* dst = p.out + ((int64_t)(row0 + qi) * p.n_q + (kvh * p.R + r)) * kDT;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t a[32], b[32];
-        ptx::tmem_ld_32x32b_x32(lane_addr + (uint32_t)(256 + c * 32), a);
-        if (n1 > 0) ptx::tmem_ld_32x32b_x32(lane_addr + (uint32_t)(384 + c * 32), b);
-        ptx::tmem_ld_wait();
-        if (valid) {
-          const float w0 = f0 * inv, w1 = f1 * inv;
-#pragma unroll
-          for (int d = 0; d < 32; d += 8) {
-            float o[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              o[e] = __uint_as_float(a[d + e]) * w0;
-              if (n1 > 0) o[e] = fmaf(use1 ? __uint_as_float(b[d + e]) : 0.f, w1, o[e]);
-            }
-            uint4 u;
-            u.x = pack2(o[0], o[1]); u.y = pack2(o[2], o[3]); u.z = pack2(o[4], o[5]); u.w = pack2(o[6], o[7]);
-            *reinterpret_cast<uint4*>(dst + c * 32 + d) = u;
-          }
-        }
-      }
-      if (kContig && valid && p.lse != nullptr)
-        p.lse[(int64_t)(row0 + qi) * p.n_q + (kvh * p.R + r)] = m_all + log2f(l_tot);
-    }
-  }
-
-  ptx::tc_fence_before_sync();
-  ptx::cluster_sync();
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc(tmem_base, 512);
-  }
-}
-
+int g_fwd_generation = 2;       // prl_attn_varlen_fwd / _fwd_kv
+int g_prefill_generation = 2;   // prl_paged_attn_prefill_tc
 
 }  // namespace
 }  // namespace prl
 
 using namespace prl;
 
-// which forward kernel the two entry points launch (generation 1 stays selectable for A/B runs and tests:
-// PRL_ATTN_FWD=1 / PRL_PREFILL_ATTN_GEN=1, prl_attn_set_fwd_generation / prl_attn_set_prefill_generation)
-namespace prl { namespace {
-int g_fwd_generation = [] { const char* e = getenv("PRL_ATTN_FWD"); return (e && e[0] == '1') ? 1 : 2; }();
-int g_prefill_generation = [] { const char* e = getenv("PRL_PREFILL_ATTN_GEN"); return (e && e[0] == '1') ? 1 : 2; }();
-} }
+extern "C" int prl_attn_set_fwd_generation(int32_t gen) {
+  PRL_CHECK_ARG(gen == 1 || gen == 2, "prl_attn_set_fwd_generation: 1 (rescale every step) or 2 (rescale past 2^8)");
+  prl::g_fwd_generation = gen;
+  return PRL_OK;
+}
 
 extern "C" int prl_attn_set_prefill_generation(int32_t gen) {
-  PRL_CHECK_ARG(gen == 1 || gen == 2, "prl_attn_set_prefill_generation: 1 or 2");
+  PRL_CHECK_ARG(gen == 1 || gen == 2, "prl_attn_set_prefill_generation: 1 (rescale every step) or 2 (rescale past 2^8)");
   prl::g_prefill_generation = gen;
   return PRL_OK;
 }
@@ -690,43 +298,19 @@ extern "C" int prl_paged_attn_prefill_tc(const void* q, int32_t q_rows, const vo
   p.seq_slot = seq_slot; p.seq_kv_start = nullptr; p.max_blocks = max_blocks; p.n_q = n_q; p.n_kv = n_kv; p.R = n_q / n_kv;
   p.nq = 128 / p.R;
   p.n_pages = n_pages; p.layer = layer; p.scale_log2 = sm_scale * 1.4426950408889634f;
-  p.col_k = p.col_v = 0; p.lse = nullptr; p.timing = nullptr;
+  p.col_k = p.col_v = 0; p.lse = nullptr;
   CUtensorMap tq, tkv;
   int rc = make_tmap_2d_bf16(&tkv, kv_cache, kDT, (uint64_t)total_rows, kDT * 2, 64, kPageT);
   if (rc) return rc;
   rc = make_tmap_3d_bf16(&tq, q, kDT, (uint64_t)n_q, (uint64_t)q_rows, kDT * 2, (uint64_t)n_q * kDT * 2, 64, (uint32_t)p.R,
                          (uint32_t)p.nq);
   if (rc) return rc;
-  const int smem = 2 * kTile16K + 2 * kStageBytesT + 4 * kTile16K + 1024 + 8 * 20 + 2 * 128 * 4 + 16;
-  static SmemAttr smem_attr = {};
-  dim3 grid((unsigned)(((max_q_len + p.nq - 1) / p.nq + 1) & ~1), (unsigned)n_kv, (unsigned)n_seqs);  // pairs of q tiles
-  if (g_prefill_generation == 2) {      // ping-pong softmax groups, P and O in TMEM (see attn_fwd_v2_kernel)
-    static SmemAttr smem_attr2 = {};
-    PRL_CUDA(ensure_smem(attn_fwd_v2_kernel<false>, smem, smem_attr2));
-    attn_fwd_v2_kernel<false><<<grid, kThreadsT, (size_t)smem, (cudaStream_t)stream_>>>(tq, tkv, p);
-  } else {
-    PRL_CUDA(ensure_smem(attn_prefill_tc_kernel<false>, smem, smem_attr));
-    attn_prefill_tc_kernel<false><<<grid, kThreadsT, (size_t)smem, (cudaStream_t)stream_>>>(tq, tkv, p);
-  }
+  dim3 grid((unsigned)((max_q_len + p.nq - 1) / p.nq), (unsigned)n_kv, (unsigned)n_seqs);
+  PRL_CUDA(launch_fwd<false>(g_prefill_generation, grid, tq, tkv, p, (cudaStream_t)stream_));
   PRL_LAUNCH_CHECK();
   return PRL_OK;
 }
 
-
-namespace prl { namespace { long long* g_fwd_timing = nullptr; } }
-// measurement only: per-phase cycle sums of CTA (0,0,0) of the next generation-2 learner forward launches
-// [0..5] group 0: wait S | tcgen05.ld | mask + max | wait O + rescale | exp2 + pack + tcgen05.st | barrier + arrive
-// [8..13] group 1 likewise; [16] MMA warp waiting for P, [17] for V, [18] MMA warp total, [19] steps.  NULL switches it off.
-extern "C" int prl_attn_debug_timing(int64_t* out20_device) {
-  prl::g_fwd_timing = (long long*)out20_device;
-  return PRL_OK;
-}
-
-extern "C" int prl_attn_set_fwd_generation(int32_t gen) {
-  PRL_CHECK_ARG(gen == 1 || gen == 2, "prl_attn_set_fwd_generation: 1 (lock-step softmax, O folded in registers) or 2 (ping-pong, O in TMEM)");
-  prl::g_fwd_generation = gen;
-  return PRL_OK;
-}
 
 // Learner forward (hot path 2): block-diagonal causal attention over ONE packed row, the varlen flash-attention call
 // the reference makes through HF (pipelinerl/finetune/rl/__init__.py:204 with packed position_ids,
@@ -747,28 +331,15 @@ extern "C" int prl_attn_varlen_fwd(const void* qkv, int64_t qkv_stride, int32_t 
   p.block_table = nullptr; p.seq_q_start = seg_start; p.seq_q_len = seg_len; p.seq_pos0 = nullptr; p.seq_slot = nullptr; p.seq_kv_start = nullptr;
   p.max_blocks = 0; p.n_q = n_q; p.n_kv = n_kv; p.R = n_q / n_kv; p.nq = 128 / p.R;
   p.n_pages = 0; p.layer = 0; p.scale_log2 = sm_scale * 1.4426950408889634f;
-  p.col_k = n_q * kDT; p.col_v = (n_q + n_kv) * kDT; p.lse = lse; p.timing = g_fwd_timing;
+  p.col_k = n_q * kDT; p.col_v = (n_q + n_kv) * kDT; p.lse = lse;
   CUtensorMap tq, tkv;
   int rc = make_tmap_2d_bf16(&tkv, qkv, (uint64_t)(n_q + 2 * n_kv) * kDT, (uint64_t)T, (uint64_t)qkv_stride * 2, 64, kPageT);
   if (rc) return rc;
   rc = make_tmap_3d_bf16(&tq, qkv, kDT, (uint64_t)n_q, (uint64_t)T, kDT * 2, (uint64_t)qkv_stride * 2, 64, (uint32_t)p.R,
                          (uint32_t)p.nq);
   if (rc) return rc;
-  const int smem = 2 * kTile16K + 2 * kStageBytesT + 4 * kTile16K + 1024 + 8 * 20 + 2 * 128 * 4 + 16;
-  dim3 grid((unsigned)(((max_seg_len + p.nq - 1) / p.nq + 1) & ~1), (unsigned)n_kv, (unsigned)n_seg);
-  if (g_fwd_generation == 1) {      // A/B and tests only (prl_attn_set_fwd_generation)
-    static SmemAttr smem_attr = {};
-    PRL_CUDA(ensure_smem(attn_prefill_tc_kernel<true>, smem, smem_attr));
-    attn_prefill_tc_kernel<true><<<grid, kThreadsT, (size_t)smem, (cudaStream_t)stream_>>>(tq, tkv, p);
-  } else if (g_fwd_timing != nullptr) {
-    static SmemAttr smem_attr_t = {};
-    PRL_CUDA(ensure_smem(attn_fwd_v2_kernel<true, true>, smem, smem_attr_t));
-    attn_fwd_v2_kernel<true, true><<<grid, kThreadsT, (size_t)smem, (cudaStream_t)stream_>>>(tq, tkv, p);
-  } else {
-    static SmemAttr smem_attr2 = {};
-    PRL_CUDA(ensure_smem(attn_fwd_v2_kernel<true>, smem, smem_attr2));
-    attn_fwd_v2_kernel<true><<<grid, kThreadsT, (size_t)smem, (cudaStream_t)stream_>>>(tq, tkv, p);
-  }
+  dim3 grid((unsigned)((max_seg_len + p.nq - 1) / p.nq), (unsigned)n_kv, (unsigned)n_seg);
+  PRL_CUDA(launch_fwd<true>(g_fwd_generation, grid, tq, tkv, p, (cudaStream_t)stream_));
   PRL_LAUNCH_CHECK();
   return PRL_OK;
 }
@@ -795,17 +366,14 @@ extern "C" int prl_attn_varlen_fwd_kv(const void* q, int64_t q_stride, int32_t T
   p.seq_kv_start = seg_kv_start;
   p.max_blocks = 0; p.n_q = n_q; p.n_kv = n_kv; p.R = n_q / n_kv; p.nq = 128 / p.R;
   p.n_pages = 0; p.layer = 0; p.scale_log2 = sm_scale * 1.4426950408889634f;
-  p.col_k = 0; p.col_v = n_kv * kDT; p.lse = lse; p.timing = nullptr;
+  p.col_k = 0; p.col_v = n_kv * kDT; p.lse = lse;
   CUtensorMap tq, tkv;
   int rc = make_tmap_2d_bf16(&tkv, kv, (uint64_t)(2 * n_kv) * kDT, (uint64_t)Tkv, (uint64_t)kv_stride * 2, 64, kPageT);
   if (rc) return rc;
   rc = make_tmap_3d_bf16(&tq, q, kDT, (uint64_t)n_q, (uint64_t)Tq, kDT * 2, (uint64_t)q_stride * 2, 64, (uint32_t)p.R, (uint32_t)p.nq);
   if (rc) return rc;
-  const int smem = 2 * kTile16K + 2 * kStageBytesT + 4 * kTile16K + 1024 + 8 * 20 + 2 * 128 * 4 + 16;
-  dim3 grid((unsigned)(((max_q_len + p.nq - 1) / p.nq + 1) & ~1), (unsigned)n_kv, (unsigned)n_seg);
-  static SmemAttr smem_attr = {};
-  PRL_CUDA(ensure_smem(attn_fwd_v2_kernel<true>, smem, smem_attr));
-  attn_fwd_v2_kernel<true><<<grid, kThreadsT, (size_t)smem, (cudaStream_t)stream_>>>(tq, tkv, p);
+  dim3 grid((unsigned)((max_q_len + p.nq - 1) / p.nq), (unsigned)n_kv, (unsigned)n_seg);
+  PRL_CUDA(launch_fwd<true>(g_fwd_generation, grid, tq, tkv, p, (cudaStream_t)stream_));
   PRL_LAUNCH_CHECK();
   return PRL_OK;
 }

@@ -1,4 +1,4 @@
-// Hot path (1): the small fused kernels around the tcgen05 GEMMs of one token step.
+// Hot path (1): the small fused kernels around the wgmma GEMMs of one token step.
 //
 // They replace, for the reference's sampler (vLLM behind pipelinerl/async_llm.py:134),
 // vLLM's fused_add_rms_norm / rotary_embedding / reshape_and_cache_flash / silu_and_mul
@@ -483,7 +483,7 @@ extern "C" int prl_qkv_rope_cache(const float* partials, int32_t n_split, int32_
   PRL_CHECK_ARG(head_dim == 128, "prl_qkv_rope_cache: head_dim must be 128 (got %d)", head_dim);
   PRL_CHECK_ARG(B >= 1 && n_q >= 1 && n_kv >= 1 && page_size >= 1 && max_blocks >= 1, "prl_qkv_rope_cache: bad shape");
   if (B > 128) {  // prefill chunk: row-walking variant (same results, ~4x less time at 1024 rows)
-    const unsigned blocks = (unsigned)(B < 148 * 8 ? B : 148 * 8);
+    const unsigned blocks = (unsigned)(B < 132 * 8 ? B : 132 * 8);
     PRL_CUDA(launch_pdl(qkv_rope_cache_rows_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)st, partials, (int)n_split,
                         (int)B, (const __nv_bfloat16*)bias, (int)n_q, (int)n_kv, positions, block_table, (int)max_blocks,
                         row_slot, inv_freq, (__nv_bfloat16*)q_out, (__nv_bfloat16*)kv_cache, n_pages, (int)layer,

@@ -1,4 +1,4 @@
-// tcgen05 weight-streaming GEMM for the token step (hot path 1) and the output head.
+// wgmma weight-streaming GEMM for the token step (hot path 1) and the output head.
 //
 //   Y[M_tok, N_out] = X[M_tok, K] * W[N_out, K]^T      (bf16 in, fp32 accumulate)
 //
@@ -7,17 +7,16 @@
 // the fp32 lm_head matmul of pipelinerl/vllm_quantization.py:266-278.
 //
 // Decode shapes are skinny (M_tok <= 64..256), so the kernel is laid out "swap-AB":
-// the WEIGHT tile is the UMMA M operand (128 output features per CTA), the tokens are
-// the UMMA N operand (16..256), and D^T = W_tile * X^T accumulates in TMEM
-// (lane = output feature, column = token).  Every weight byte is read from HBM exactly
+// the WEIGHT tile is the wgmma M operand (128 output features per CTA, 64 per consumer
+// warpgroup), the tokens are the N operand (16..256), and D^T = W_tile * X^T accumulates in
+// registers (row = output feature, column = token).  Every weight byte is read from HBM exactly
 // once per step by TMA (EVICT_FIRST), the small activation tile is re-read from L2
-// (EVICT_LAST); split-K fills the 148 SMs when N_out/128 < #SMs, with fp32 partials
+// (EVICT_LAST); split-K fills the 132 SMs when N_out/128 < #SMs, with fp32 partials
 // reduced by the consumer epilogue kernel (decode_ops.cu) in a fixed order.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer
-// (one elected lane), warps 2..5 = epilogue (TMEM -> registers -> global).
-// An optional second weight operand W_lo (bf16 residual of an fp32 master) is
-// accumulated into the same TMEM tile: fp32-equivalent head at the cost of a second
+// Warp roles (288 threads): warps 0..7 = two consumer warpgroups (wgmma, then the epilogue),
+// warp 8 = TMA producer.  An optional second weight operand W_lo (bf16 residual of an fp32
+// master) is accumulated into the same registers: fp32-equivalent head at the cost of a second
 // bf16 stream (same bytes as an fp32 weight).
 //
 // HBM-bound: algorithmic bytes = 2*N*K (+2*N*K with W_lo) + 2*M*K + 4*split_k*M*N.
@@ -103,10 +102,10 @@ int make_tmap_3d_bf16(CUtensorMap* out, const void* base, uint64_t d0, uint64_t 
 
 namespace {
 
-constexpr int kBlockM = 128;  // output features per CTA (UMMA M)
+constexpr int kBlockM = 128;  // output features per CTA (two wgmma M = 64 halves)
 constexpr int kBlockK = 64;   // bf16 elements per stage row = 128 B = one swizzle atom
 constexpr int kUmmaK = 16;
-constexpr int kThreads = 192;
+constexpr int kThreads = 288;
 static int g_smem_budget = 100 * 1024;
 static int g_tiled_weights = 0;  // weights stored as contiguous [N/128][K/64][128][64] tiles  // per-CTA tile ring; <= 100 KB lets two CTAs share an SM
 
@@ -140,29 +139,37 @@ template <int kNTile>
 struct SmemLayout {
   static constexpr int kABytes = kBlockM * kBlockK * 2;       // 16 KB
   static constexpr int kBBytes = kNTile * kBlockK * 2;
+  static constexpr int kStageLd = kNTile + 1;                 // fp32 accumulator tile [128 features][kNTile + 1]: odd stride
+  static constexpr int kEpiBytes = kBlockM * kStageLd * 4 + 4 * kNTile * (int)sizeof(HeadPart);
   static constexpr int stage_bytes(bool lo) { return kABytes * (lo ? 2 : 1) + kBBytes; }
   static int stages(bool lo) {
     int s = g_smem_budget / stage_bytes(lo);
     return s > 8 ? 8 : (s < 2 ? 2 : s);
   }
+  // the epilogue reuses the drained tile ring for the accumulator tile (and the head statistics behind it)
+  __host__ __device__ static int ring_bytes(int n_stages, bool lo) {
+    const int r = n_stages * stage_bytes(lo);
+    return r > kEpiBytes ? r : kEpiBytes;
+  }
 };
 
+// Warp roles (288 threads): warps 0..7 = two consumer warpgroups (wgmma m64 x kNTile: warpgroup g owns weight rows
+// [64 g, 64 g + 64) of the tile, fp32 accumulators in registers), warp 8 = TMA producer.
 template <int kNTile, bool kHead>
-__global__ void __launch_bounds__(kThreads, 2)
+__global__ void __launch_bounds__(kThreads, kNTile <= 64 ? 2 : 1)
 gemm_swapab_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_wlo,
                    const __grid_constant__ CUtensorMap tm_x, GemmParams p, int n_stages) {
   using L = SmemLayout<kNTile>;
   extern __shared__ uint8_t smem_raw[];
   pdl_launch_dependents();  // let the next kernel start its own prologue / weight prefetch as early as possible
   const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* smem_gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
   const bool lo = p.has_lo != 0;
   const int stage_bytes = L::stage_bytes(lo);
   // barriers live after the tile ring
-  const uint32_t bar_base = smem_base + (uint32_t)(n_stages * stage_bytes);
+  const uint32_t bar_base = smem_base + (uint32_t)L::ring_bytes(n_stages, lo);
   auto full_bar = [&](int s) { return bar_base + 8u * (uint32_t)s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (uint32_t)(n_stages + s); };
-  const uint32_t tmem_full_bar = bar_base + 8u * (uint32_t)(2 * n_stages);
-  const uint32_t tmem_slot = tmem_full_bar + 8u;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // blockIdx.x enumerates (weight tile, token tile) with the token tile fastest, so the CTAs that share a
@@ -176,48 +183,42 @@ gemm_swapab_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_consta
   const int kb_end = (int)(((int64_t)p.kblocks * (split + 1)) / p.split_k);
   const int n_kb = kb_end - kb_begin;
 
-  // Thread 0 arms the barriers and IMMEDIATELY fills the first ring pass with WEIGHT tiles: weights do not depend on
-  // the preceding kernel (PDL lets this run under the predecessor's tail) nor on the rest of this CTA's prologue
-  // (TMEM allocation, descriptor prefetch), so the first HBM round trip overlaps both.
+  auto load_weights = [&](int i, int s) {
+    const uint32_t a_dst = smem_base + (uint32_t)(s * stage_bytes);
+    const int kcoord = (kb_begin + i) * kBlockK;
+    const int wc0 = p.tiled ? 0 : kcoord;
+    const int wc1 = p.tiled ? (n_tile * p.kblocks + kb_begin + i) * kBlockM : n0;
+    if (p.swiglu_I) {   // tm_w boxes are 64 rows here: gate half, then up half of the same 64 features
+      ptx::tma_load_2d(a_dst, &tm_w, wc0, n_tile * 64, full_bar(s), ptx::kEvictFirst);
+      ptx::tma_load_2d(a_dst + L::kABytes / 2, &tm_w, wc0, (int)p.swiglu_I + n_tile * 64, full_bar(s), ptx::kEvictFirst);
+    } else {
+      ptx::tma_load_2d(a_dst, &tm_w, wc0, wc1, full_bar(s), ptx::kEvictFirst);
+    }
+    if (lo) ptx::tma_load_2d(a_dst + L::kABytes, &tm_wlo, wc0, wc1, full_bar(s), ptx::kEvictFirst);
+  };
+
+  // The producer thread arms the barriers and IMMEDIATELY fills the first ring pass with WEIGHT tiles: weights do not
+  // depend on the preceding kernel (PDL lets this run under the predecessor's tail), so the first HBM round trip
+  // overlaps the predecessor's tail and this CTA's prologue.
   const int pre = n_kb < n_stages ? n_kb : n_stages;
-  if (threadIdx.x == 0) {
+  if (threadIdx.x == 256) {
     for (int s = 0; s < n_stages; ++s) {
       ptx::mbar_init(full_bar(s), 1);
-      ptx::mbar_init(empty_bar(s), 1);
+      ptx::mbar_init(empty_bar(s), 2);   // one elected thread of each consumer warpgroup
     }
-    ptx::mbar_init(tmem_full_bar, 1);
     ptx::fence_barrier_init();
     ptx::fence_proxy_async();
     for (int i = 0; i < pre; ++i) {
       ptx::mbar_arrive_expect_tx(full_bar(i), (uint32_t)stage_bytes);
-      const uint32_t a_dst = smem_base + (uint32_t)(i * stage_bytes);
-      const int kcoord = (kb_begin + i) * kBlockK;
-      const int wc0 = p.tiled ? 0 : kcoord;
-      const int wc1 = p.tiled ? (n_tile * p.kblocks + kb_begin + i) * kBlockM : n0;
-      if (p.swiglu_I) {   // tm_w boxes are 64 rows here: gate half, then up half of the same 64 features
-        ptx::tma_load_2d(a_dst, &tm_w, wc0, n_tile * 64, full_bar(i), ptx::kEvictFirst);
-        ptx::tma_load_2d(a_dst + L::kABytes / 2, &tm_w, wc0, (int)p.swiglu_I + n_tile * 64, full_bar(i), ptx::kEvictFirst);
-      } else {
-        ptx::tma_load_2d(a_dst, &tm_w, wc0, wc1, full_bar(i), ptx::kEvictFirst);
-      }
-      if (lo) ptx::tma_load_2d(a_dst + L::kABytes, &tm_wlo, wc0, wc1, full_bar(i), ptx::kEvictFirst);
+      load_weights(i, i);
     }
     ptx::prefetch_tensormap(&tm_x);
   }
-  if (warp == 1) {
-    ptx::tmem_alloc(tmem_slot, kNTile < 32 ? 32 : kNTile);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before_sync();
   __syncthreads();
-  ptx::tc_fence_after_sync();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp == 0) {
-    // ===== TMA producer =====  (first-pass weight tiles were issued by thread 0 before the CTA-wide sync)
+  if (warp == 8) {
+    // ===== TMA producer =====  (first-pass weight tiles were issued before the CTA-wide sync)
     if (lane == 0) {
-      const uint32_t tx = (uint32_t)stage_bytes;
       pdl_wait();
       for (int i = 0; i < pre; ++i) {
         const uint32_t b_dst = smem_base + (uint32_t)(i * stage_bytes) + L::kABytes * (lo ? 2 : 1);
@@ -227,184 +228,137 @@ gemm_swapab_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_consta
         const int s = i % n_stages;
         const uint32_t ph = (uint32_t)((i / n_stages) & 1);
         ptx::mbar_wait(empty_bar(s), ph ^ 1u);
-        ptx::mbar_arrive_expect_tx(full_bar(s), tx);
-        const uint32_t a_dst = smem_base + (uint32_t)(s * stage_bytes);
-        const int kcoord = (kb_begin + i) * kBlockK;
-        const int wc0 = p.tiled ? 0 : kcoord;
-        const int wc1 = p.tiled ? (n_tile * p.kblocks + kb_begin + i) * kBlockM : n0;
-        if (p.swiglu_I) {
-          ptx::tma_load_2d(a_dst, &tm_w, wc0, n_tile * 64, full_bar(s), ptx::kEvictFirst);
-          ptx::tma_load_2d(a_dst + L::kABytes / 2, &tm_w, wc0, (int)p.swiglu_I + n_tile * 64, full_bar(s), ptx::kEvictFirst);
-        } else {
-          ptx::tma_load_2d(a_dst, &tm_w, wc0, wc1, full_bar(s), ptx::kEvictFirst);
-        }
-        uint32_t b_dst = a_dst + L::kABytes;
-        if (lo) {
-          ptx::tma_load_2d(a_dst + L::kABytes, &tm_wlo, wc0, wc1, full_bar(s), ptx::kEvictFirst);
-          b_dst += L::kABytes;
-        }
-        ptx::tma_load_2d(b_dst, &tm_x, kcoord, m0, full_bar(s), ptx::kEvictLast);
+        ptx::mbar_arrive_expect_tx(full_bar(s), (uint32_t)stage_bytes);
+        load_weights(i, s);
+        const uint32_t b_dst = smem_base + (uint32_t)(s * stage_bytes) + L::kABytes * (lo ? 2 : 1);
+        ptx::tma_load_2d(b_dst, &tm_x, (kb_begin + i) * kBlockK, m0, full_bar(s), ptx::kEvictLast);
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      constexpr uint32_t idesc = ptx::make_idesc_bf16_f32(kBlockM, kNTile);
-      for (int i = 0; i < n_kb; ++i) {
-        const int s = i % n_stages;
-        const uint32_t ph = (uint32_t)((i / n_stages) & 1);
-        ptx::mbar_wait(full_bar(s), ph);
-        ptx::tc_fence_after_sync();
-        const uint32_t a_addr = smem_base + (uint32_t)(s * stage_bytes);
-        const uint32_t b_addr = a_addr + L::kABytes * (lo ? 2 : 1);
-        const uint64_t a_desc = ptx::make_kmajor_sw128_desc(a_addr);
-        const uint64_t b_desc = ptx::make_kmajor_sw128_desc(b_addr);
+    return;
+  }
+
+  // ===== consumers: warpgroup wg = weight rows [64 wg, 64 wg + 64), all kNTile tokens =====
+  const int wg = warp >> 2;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  float acc[kNTile / 2];
 #pragma unroll
-        for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-          // advancing K by 16 bf16 = 32 B inside the 128-B swizzle atom: +2 in the (addr >> 4) field
-          ptx::mma_bf16_ss(tmem_base, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), idesc,
-                           (i > 0 || k > 0) ? 1u : 0u);
-        }
-        if (lo) {
-          const uint64_t al_desc = ptx::make_kmajor_sw128_desc(a_addr + L::kABytes);
+  for (int e = 0; e < kNTile / 2; ++e) acc[e] = 0.f;
+  for (int i = 0; i < n_kb; ++i) {
+    const int s = i % n_stages;
+    ptx::mbar_wait(full_bar(s), (uint32_t)((i / n_stages) & 1));
+    const uint32_t a_addr = smem_base + (uint32_t)(s * stage_bytes) + (uint32_t)(wg * 64 * 128);
+    const uint32_t b_addr = smem_base + (uint32_t)(s * stage_bytes) + L::kABytes * (lo ? 2 : 1);
+    const uint64_t a_desc = ptx::make_kmajor_sw128_desc(a_addr);
+    const uint64_t b_desc = ptx::make_kmajor_sw128_desc(b_addr);
+    ptx::fence_acc(acc);
+    ptx::wg_fence();
 #pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k)
-            ptx::mma_bf16_ss(tmem_base, al_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), idesc, 1u);
-        }
-        ptx::tc_commit(empty_bar(s));  // frees the smem slot when these MMAs have read it
-      }
-      ptx::tc_commit(tmem_full_bar);   // accumulator complete
+    for (int k = 0; k < kBlockK / kUmmaK; ++k)
+      ptx::wgmma_ss<0, 0>(acc, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), 1u);
+    if (lo) {
+      const uint64_t al_desc = ptx::make_kmajor_sw128_desc(a_addr + L::kABytes);
+#pragma unroll
+      for (int k = 0; k < kBlockK / kUmmaK; ++k)
+        ptx::wgmma_ss<0, 0>(acc, al_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), 1u);
     }
-    __syncwarp();
-  } else {
-    // ===== epilogue =====
-    pdl_wait();  // the output buffers may still be read by the predecessor's consumer
-    ptx::mbar_wait(tmem_full_bar, 0);
-    ptx::tc_fence_after_sync();
-    const int q = warp & 3;                    // TMEM lane quarter this warp may read
-    const int feat = n0 + q * 32 + lane;       // output feature (vocab id) owned by this thread
-    const int m_valid = (int)((p.M - m0) < kNTile ? (p.M - m0) : kNTile);
-    const bool feat_ok = feat < p.N;
-    constexpr int kChunk = kNTile < 32 ? 16 : 32;
-    if constexpr (!kHead) {
-      if (p.swiglu_I) {
-        // ---- SwiGLU: accumulator rows 0..63 = gate, 64..127 = up of features [64 t, 64 t + 64); columns = tokens.  The up
-        //      half crosses to the gate half's threads through shared memory (the tile ring is drained), token-major so
-        //      that both the stores and the loads are conflict-free ----
-        float* xch = reinterpret_cast<float*>(smem_raw + (smem_base - ptx::smem_u32(smem_raw)));   // [kNTile][64]
-        const int r = (q & 1) * 32 + lane;             // feature inside the 64
-#pragma unroll 1
-        for (int c0 = 0; c0 < kNTile; c0 += kChunk) {
-          uint32_t v[kChunk];
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-          if constexpr (kChunk == 32) ptx::tmem_ld_32x32b_x32(taddr, v);
-          else ptx::tmem_ld_32x32b_x16(taddr, v);
-          ptx::tmem_ld_wait();
-          if (q >= 2) {
+    ptx::wg_commit();
+    ptx::wg_wait<1>();                       // the previous stage's wgmmas are done: release that slot
+    if (i > 0 && wg_leader) ptx::mbar_arrive(empty_bar((i - 1) % n_stages));
+  }
+  ptx::wg_wait<0>();
+  ptx::fence_acc(acc);
+
+  // ---- accumulators -> fp32 tile [feature][token] in the drained ring (every stage has been waited on) ----
+  asm volatile("bar.sync 1, 256;" ::: "memory");   // both warpgroups are past their last shared-memory operand read
+  float* stile = reinterpret_cast<float*>(smem_gen);
+  {
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-            for (int j = 0; j < kChunk; ++j) xch[(c0 + j) * 64 + r] = __uint_as_float(v[j]);
-          }
-          asm volatile("bar.sync 1, 128;" ::: "memory");
-          if (q < 2) {
-            const int64_t f = (int64_t)n_tile * 64 + r;
-#pragma unroll
-            for (int j = 0; j < kChunk; ++j) {
-              if (c0 + j < m_valid) {
-                const float gg = __uint_as_float(v[j]), uu = xch[(c0 + j) * 64 + r];
-                p.act[(int64_t)(m0 + c0 + j) * p.swiglu_I + f] = __float2bfloat16_rn((gg / (1.f + __expf(-gg))) * uu);
-              }
-            }
-          }
-          asm volatile("bar.sync 1, 128;" ::: "memory");   // xch is rewritten by the next chunk
+    for (int j = 0; j < kNTile / 8; ++j) {
+      const int c = 8 * j + 2 * (lane & 3);
+      stile[r0 * L::kStageLd + c] = acc[4 * j];
+      stile[r0 * L::kStageLd + c + 1] = acc[4 * j + 1];
+      stile[(r0 + 8) * L::kStageLd + c] = acc[4 * j + 2];
+      stile[(r0 + 8) * L::kStageLd + c + 1] = acc[4 * j + 3];
+    }
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+
+  // ===== epilogue: thread = one output feature (lanes = 32 consecutive features), half of the tokens =====
+  pdl_wait();  // the output buffers may still be read by the predecessor's consumer
+  const int q = warp & 3;                    // feature quarter
+  const int half = warp >> 2;                // token half
+  const int fr = q * 32 + lane;              // tile row
+  const int feat = n0 + fr;                  // output feature (vocab id) owned by this thread
+  const int m_valid = (int)((p.M - m0) < kNTile ? (p.M - m0) : kNTile);
+  const bool feat_ok = feat < p.N;
+  constexpr int kHalfTok = kNTile / 2;
+  const int tb = half * kHalfTok, te = tb + kHalfTok;
+  const float* srow = stile + fr * L::kStageLd;
+  if constexpr (!kHead) {
+    if (p.swiglu_I) {
+      // ---- SwiGLU: tile rows 0..63 = gate, 64..127 = up of features [64 t, 64 t + 64); columns = tokens ----
+      if (q < 2) {
+        const int64_t f = (int64_t)n_tile * 64 + fr;
+        const float* urow = stile + (fr + 64) * L::kStageLd;
+        for (int t = tb; t < te && t < m_valid; ++t) {
+          const float gg = srow[t], uu = urow[t];
+          p.act[(int64_t)(m0 + t) * p.swiglu_I + f] = __float2bfloat16_rn((gg / (1.f + __expf(-gg))) * uu);
         }
-      } else {
-      // ---- TMEM -> registers -> fp32 partial tile ----
+      }
+    } else if (feat_ok) {
+      // ---- fp32 partial tile: 32 lanes -> one 128-B row segment per token ----
       float* out = p.partials + ((int64_t)split * p.M + m0) * p.N + feat;
       // tensor-parallel row-parallel GEMM: the partial sums are ALSO stored straight into the peer GPU's reduction
       // buffer over NVLink, so the "all-reduce" is this epilogue plus the consumer's ordinary split reduction
       float* out_peer = p.peer_partials ? p.peer_partials + ((int64_t)split * p.M + m0) * p.N + feat : nullptr;
-#pragma unroll 1
-      for (int c0 = 0; c0 < kNTile; c0 += kChunk) {
-        uint32_t r[kChunk];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-        if constexpr (kChunk == 32) ptx::tmem_ld_32x32b_x32(taddr, r);
-        else ptx::tmem_ld_32x32b_x16(taddr, r);
-        ptx::tmem_ld_wait();
-        if (n_kb == 0) {
-#pragma unroll
-          for (int j = 0; j < kChunk; ++j) r[j] = 0u;
-        }
-        if (feat_ok) {
-#pragma unroll
-          for (int j = 0; j < kChunk; ++j)
-            if (c0 + j < m_valid) out[(int64_t)(c0 + j) * p.N] = __uint_as_float(r[j]);  // 32 lanes -> 128 B row segment
-          if (out_peer) {
-#pragma unroll
-            for (int j = 0; j < kChunk; ++j)
-              if (c0 + j < m_valid) out_peer[(int64_t)(c0 + j) * p.N] = __uint_as_float(r[j]);
-          }
-        }
-      }
-      }
-    } else {
-      // ---- fused output head: per token, online-softmax statistics over this tile's 128 vocabulary rows,
-      //      the target logit and the best Gumbel-perturbed logit; the logits themselves are never stored ----
-      HeadPart* s_hp = reinterpret_cast<HeadPart*>(smem_raw + (smem_base - ptx::smem_u32(smem_raw)));  // [4][kNTile], ring is drained
-#pragma unroll 1
-      for (int c0 = 0; c0 < kNTile; c0 += kChunk) {
-        uint32_t r[kChunk];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-        if constexpr (kChunk == 32) ptx::tmem_ld_32x32b_x32(taddr, r);
-        else ptx::tmem_ld_32x32b_x16(taddr, r);
-        ptx::tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < kChunk; ++j) {
-          const int tok = m0 + c0 + j;
-          const bool tok_ok = c0 + j < m_valid;
-          const float z = feat_ok ? __uint_as_float(r[j]) * p.inv_temp : -INFINITY;
-          const float m = warp_max(z);
-          const float e = (z == -INFINITY) ? 0.f : __expf(z - m);
-          const float ssum = warp_sum(e);
-          const float usum = warp_sum(e > 0.f ? e * z : 0.f);
-          float key = -INFINITY;
-          if (feat_ok) key = p.greedy ? z : z + gumbel(p.seed, p.step, (uint32_t)tok, (uint32_t)feat);
-          float bkey = key, bz = z;
-          int bidx = feat_ok ? feat : 0x7fffffff;
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) {
-            const float k2 = __shfl_xor_sync(0xffffffffu, bkey, o);
-            const float z2 = __shfl_xor_sync(0xffffffffu, bz, o);
-            const int i2 = __shfl_xor_sync(0xffffffffu, bidx, o);
-            if (k2 > bkey || (k2 == bkey && i2 < bidx)) { bkey = k2; bz = z2; bidx = i2; }
-          }
-          if (p.targets && tok_ok && feat_ok && p.targets[tok] == (int64_t)feat) p.picked[tok] = z;
-          if (lane == 0) s_hp[q * kNTile + c0 + j] = HeadPart{m, ssum, usum, bkey, bz, bidx};
-        }
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");  // the four epilogue warps only
-      const int et = threadIdx.x - 64;                // 0..127
-      for (int tkn = et; tkn < m_valid; tkn += 128) {
-        HeadPart a = s_hp[tkn];
-#pragma unroll
-        for (int qq = 1; qq < 4; ++qq) {
-          const HeadPart b = s_hp[qq * kNTile + tkn];
-          const float mm = fmaxf(a.m, b.m);
-          const float fa = (a.m == -INFINITY) ? 0.f : __expf(a.m - mm), fb = (b.m == -INFINITY) ? 0.f : __expf(b.m - mm);
-          a.s = a.s * fa + b.s * fb;
-          a.u = a.u * fa + b.u * fb;
-          a.m = mm;
-          if (b.key > a.key || (b.key == a.key && b.idx < a.idx)) { a.key = b.key; a.z = b.z; a.idx = b.idx; }
-        }
-        p.head_part[(int64_t)n_tile * p.M + m0 + tkn] = a;
+      for (int t = tb; t < te && t < m_valid; ++t) {
+        out[(int64_t)t * p.N] = srow[t];
+        if (out_peer) out_peer[(int64_t)t * p.N] = srow[t];
       }
     }
-  }
-
-  ptx::tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc(tmem_base, kNTile < 32 ? 32 : kNTile);
+  } else {
+    // ---- fused output head: per token, online-softmax statistics over this tile's 128 vocabulary rows,
+    //      the target logit and the best Gumbel-perturbed logit; the logits themselves are never stored ----
+    HeadPart* s_hp = reinterpret_cast<HeadPart*>(smem_gen + kBlockM * L::kStageLd * 4);  // [4][kNTile]
+#pragma unroll 1
+    for (int t = tb; t < te; ++t) {
+      const int tok = m0 + t;
+      const bool tok_ok = t < m_valid;
+      const float z = feat_ok ? srow[t] * p.inv_temp : -INFINITY;
+      const float m = warp_max(z);
+      const float e = (z == -INFINITY) ? 0.f : __expf(z - m);
+      const float ssum = warp_sum(e);
+      const float usum = warp_sum(e > 0.f ? e * z : 0.f);
+      float key = -INFINITY;
+      if (feat_ok) key = p.greedy ? z : z + gumbel(p.seed, p.step, (uint32_t)tok, (uint32_t)feat);
+      float bkey = key, bz = z;
+      int bidx = feat_ok ? feat : 0x7fffffff;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const float k2 = __shfl_xor_sync(0xffffffffu, bkey, o);
+        const float z2 = __shfl_xor_sync(0xffffffffu, bz, o);
+        const int i2 = __shfl_xor_sync(0xffffffffu, bidx, o);
+        if (k2 > bkey || (k2 == bkey && i2 < bidx)) { bkey = k2; bz = z2; bidx = i2; }
+      }
+      if (p.targets && tok_ok && feat_ok && p.targets[tok] == (int64_t)feat) p.picked[tok] = z;
+      if (lane == 0) s_hp[q * kNTile + t] = HeadPart{m, ssum, usum, bkey, bz, bidx};
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");  // the consumer warps only
+    for (int tkn = threadIdx.x; tkn < m_valid; tkn += 256) {
+      HeadPart a = s_hp[tkn];
+#pragma unroll
+      for (int qq = 1; qq < 4; ++qq) {
+        const HeadPart b = s_hp[qq * kNTile + tkn];
+        const float mm = fmaxf(a.m, b.m);
+        const float fa = (a.m == -INFINITY) ? 0.f : __expf(a.m - mm), fb = (b.m == -INFINITY) ? 0.f : __expf(b.m - mm);
+        a.s = a.s * fa + b.s * fb;
+        a.u = a.u * fa + b.u * fb;
+        a.m = mm;
+        if (b.key > a.key || (b.key == a.key && b.idx < a.idx)) { a.key = b.key; a.z = b.z; a.idx = b.idx; }
+      }
+      p.head_part[(int64_t)n_tile * p.M + m0 + tkn] = a;
+    }
   }
 }
 
@@ -453,156 +407,13 @@ int launch_gemm(const CUtensorMap& tw, const CUtensorMap& twl, const CUtensorMap
     if (n_stages > 8) n_stages = 8;
     if (n_stages < 2) n_stages = 2;
   }
-  const int smem = n_stages * L::stage_bytes(lo) + 1024 /*align slack*/ + 8 * (2 * n_stages + 2) + 16;
+  const int smem = L::ring_bytes(n_stages, lo) + 1024 /*align slack*/ + 8 * (2 * n_stages) + 16;
   auto kernel = p.head ? gemm_swapab_kernel<kNTile, true> : gemm_swapab_kernel<kNTile, false>;
   static SmemAttr smem_attr[2] = {};
   PRL_CUDA(ensure_smem(kernel, smem, smem_attr[p.head ? 1 : 0]));
   const int64_t feat_tiles = p.swiglu_I ? p.swiglu_I / 64 : (p.N + kBlockM - 1) / kBlockM;
   dim3 grid((unsigned)(feat_tiles * ((p.M + kNTile - 1) / kNTile)), (unsigned)p.split_k, 1);
   PRL_CUDA(launch_pdl(kernel, grid, dim3(kThreads), (size_t)smem, stream, tw, twl, tx, p, n_stages));
-  PRL_LAUNCH_CHECK();
-  return PRL_OK;
-}
-
-// ------------------------------------------------------------------------------------
-// CTA-pair variant for compute-bound shapes (chunked prefill, scoring, learner forward: M_tok > 128).
-// A (2,1,1) cluster owns a 256-feature x 256-token output tile: each CTA stages its own 128 weight rows and
-// 128 of the 256 token rows per k-block (32 KB/stage/CTA instead of 48 KB for the same math), the leader issues
-// ONE tcgen05.mma.cta_group::2 (UMMA 256x256x16) per K=16 slice, and each CTA's TMEM receives the 128 features
-// it staged x all 256 tokens.  Per-SM shared-memory operand traffic per flop is halved relative to cta_group::1.
-// ------------------------------------------------------------------------------------
-constexpr int k2TokTile = 256;                       // tokens per CTA pair (UMMA N)
-constexpr int k2StageBytes = 2 * kBlockM * kBlockK * 2;  // 16 KB weights + 16 KB tokens per CTA
-static int g_use_2cta = 1;
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-gemm_pair_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x, GemmParams p,
-                 int n_stages) {
-  extern __shared__ uint8_t smem_raw[];
-  pdl_launch_dependents();
-  const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + (uint32_t)(n_stages * k2StageBytes);
-  auto full_bar = [&](int s) { return bar_base + 8u * (uint32_t)s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (uint32_t)(n_stages + s); };
-  const uint32_t tmem_full_bar = bar_base + 8u * (uint32_t)(2 * n_stages);
-  const uint32_t tmem_slot = tmem_full_bar + 8u;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = ptx::cluster_ctarank();
-  const int pair = (int)blockIdx.x >> 1;
-  const int m_tiles = (int)((p.M + k2TokTile - 1) / k2TokTile);
-  const int n0 = (pair / m_tiles) * (2 * kBlockM) + (int)rank * kBlockM;  // first output feature of THIS CTA
-  const int m0 = (pair % m_tiles) * k2TokTile;                            // first token of the pair
-  const int split = blockIdx.y;
-  const int kb_begin = (int)(((int64_t)p.kblocks * split) / p.split_k);
-  const int kb_end = (int)(((int64_t)p.kblocks * (split + 1)) / p.split_k);
-  const int n_kb = kb_end - kb_begin;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < n_stages; ++s) {
-      ptx::mbar_init(full_bar(s), 2);   // leader's arrive.expect_tx + the peer's remote arrive (only rank 0's copy is used)
-      ptx::mbar_init(empty_bar(s), 1);  // multicast tcgen05.commit
-    }
-    ptx::mbar_init(tmem_full_bar, 1);
-    ptx::fence_barrier_init();
-    ptx::fence_proxy_async();
-    ptx::prefetch_tensormap(&tm_w);
-    ptx::prefetch_tensormap(&tm_x);
-  }
-  ptx::cluster_sync();  // both CTAs' barriers exist before any remote arrive / TMA completion / multicast commit
-  if (warp == 1) {
-    ptx::tmem_alloc_2sm(tmem_slot, k2TokTile);
-    ptx::tmem_relinquish_2sm();
-  }
-  ptx::tc_fence_before_sync();
-  ptx::cluster_sync();
-  ptx::tc_fence_after_sync();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-
-  if (warp == 0) {
-    // ===== TMA producer (both CTAs) =====
-    if (lane == 0) {
-      pdl_wait();
-      const uint64_t w_hint = m_tiles > 1 ? ptx::kEvictNormal : ptx::kEvictFirst;  // token tiles re-read the weights via L2
-      for (int i = 0; i < n_kb; ++i) {
-        const int s = i % n_stages;
-        const uint32_t ph = (uint32_t)((i / n_stages) & 1);
-        ptx::mbar_wait(empty_bar(s), ph ^ 1u);
-        if (rank == 0) ptx::mbar_arrive_expect_tx(full_bar(s), 2u * (uint32_t)k2StageBytes);
-        else ptx::mbar_arrive_remote(full_bar(s), 0);
-        const uint32_t a_dst = smem_base + (uint32_t)(s * k2StageBytes);
-        const int kcoord = (kb_begin + i) * kBlockK;
-        ptx::tma_load_2d_2sm(a_dst, &tm_w, kcoord, n0, full_bar(s), w_hint);
-        ptx::tma_load_2d_2sm(a_dst + kBlockM * kBlockK * 2, &tm_x, kcoord, m0 + (int)rank * kBlockM, full_bar(s),
-                             ptx::kEvictLast);
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer (leader CTA only) =====
-    if (lane == 0 && rank == 0) {
-      constexpr uint32_t idesc = ptx::make_idesc_bf16_f32(2 * kBlockM, k2TokTile);
-      for (int i = 0; i < n_kb; ++i) {
-        const int s = i % n_stages;
-        const uint32_t ph = (uint32_t)((i / n_stages) & 1);
-        ptx::mbar_wait(full_bar(s), ph);
-        ptx::tc_fence_after_sync();
-        const uint32_t a_addr = smem_base + (uint32_t)(s * k2StageBytes);
-        const uint64_t a_desc = ptx::make_kmajor_sw128_desc(a_addr);
-        const uint64_t b_desc = ptx::make_kmajor_sw128_desc(a_addr + kBlockM * kBlockK * 2);
-#pragma unroll
-        for (int k = 0; k < kBlockK / kUmmaK; ++k)
-          ptx::mma_bf16_ss_2sm(tmem_base, a_desc + (uint64_t)(2 * k), b_desc + (uint64_t)(2 * k), idesc,
-                               (i > 0 || k > 0) ? 1u : 0u);
-        ptx::tc_commit_2sm(empty_bar(s), 3);  // both CTAs' slots
-      }
-      ptx::tc_commit_2sm(tmem_full_bar, 3);
-    }
-    __syncwarp();
-  } else {
-    // ===== epilogue (both CTAs: 128 features x 256 tokens each) =====
-    pdl_wait();
-    ptx::mbar_wait(tmem_full_bar, 0);
-    ptx::tc_fence_after_sync();
-    const int q = warp & 3;
-    const int feat = n0 + q * 32 + lane;
-    const int m_valid = (int)((p.M - m0) < k2TokTile ? (p.M - m0) : k2TokTile);
-    const bool feat_ok = feat < p.N;
-    float* out = p.partials + ((int64_t)split * p.M + m0) * p.N + feat;
-#pragma unroll 1
-    for (int c0 = 0; c0 < k2TokTile; c0 += 32) {
-      if (c0 >= m_valid) break;
-      uint32_t r[32];
-      ptx::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, r);
-      ptx::tmem_ld_wait();
-      if (n_kb == 0) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = 0u;
-      }
-      if (feat_ok) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (c0 + j < m_valid) out[(int64_t)(c0 + j) * p.N] = __uint_as_float(r[j]);
-      }
-    }
-  }
-
-  ptx::tc_fence_before_sync();
-  ptx::cluster_sync();  // neither CTA may release TMEM (or exit) while the pair's MMAs / the peer's reads are in flight
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc_2sm(tmem_base, k2TokTile);
-  }
-}
-
-int launch_gemm_pair(const CUtensorMap& tw, const CUtensorMap& tx, const GemmParams& p, cudaStream_t stream) {
-  int n_stages = 6;
-  const int smem = n_stages * k2StageBytes + 1024 + 8 * (2 * n_stages + 2) + 16;
-  static SmemAttr smem_attr = {};
-  PRL_CUDA(ensure_smem(gemm_pair_kernel, smem, smem_attr));
-  const int64_t pairs = ((p.N + 2 * kBlockM - 1) / (2 * kBlockM)) * ((p.M + k2TokTile - 1) / k2TokTile);
-  dim3 grid((unsigned)(2 * pairs), (unsigned)p.split_k, 1);
-  PRL_CUDA(launch_pdl(gemm_pair_kernel, grid, dim3(kThreads), (size_t)smem, stream, tw, tx, p, n_stages));
   PRL_LAUNCH_CHECK();
   return PRL_OK;
 }
@@ -635,11 +446,6 @@ using namespace prl;
 extern "C" int prl_gemm_set_smem_budget_kb(int32_t kb) {
   PRL_CHECK_ARG(kb >= 48 && kb <= 220, "prl_gemm_set_smem_budget_kb: 48..220 KB");
   g_smem_budget = kb * 1024;
-  return PRL_OK;
-}
-
-extern "C" int prl_gemm_set_cta_pair(int32_t on) {
-  g_use_2cta = on ? 1 : 0;
   return PRL_OK;
 }
 
@@ -729,12 +535,6 @@ static int gemm_splitk_impl(const void* W, const void* W_lo, const void* X, int6
   rc = make_tmap_2d_bf16(&tx, X, (uint64_t)K, (uint64_t)M, (uint64_t)K * 2, kBlockK, (uint32_t)nt);
   if (rc) return rc;
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (nt == 256 && g_use_2cta && !W_lo && !peer_partials && !p.tiled) {
-    // token box of 128 rows: each CTA of the pair stages half of the 256-token tile
-    rc = make_tmap_2d_bf16(&tx, X, (uint64_t)K, (uint64_t)M, (uint64_t)K * 2, kBlockK, kBlockM);
-    if (rc) return rc;
-    return launch_gemm_pair(tw, tx, p, stream);
-  }
   switch (nt) {
     case 16: return launch_gemm<16>(tw, twl, tx, p, stream);
     case 32: return launch_gemm<32>(tw, twl, tx, p, stream);
@@ -759,8 +559,8 @@ extern "C" int prl_head_logprob(const void* W, const void* W_lo, const void* X, 
   PRL_CHECK_ARG(temperature > 0.f, "prl_head_logprob: temperature must be > 0");
   PRL_CHECK_ARG(!logprob_target || targets, "prl_head_logprob: logprob_target needs targets");
   PRL_CHECK_ARG(workspace_bytes >= prl_head_workspace_bytes(M, V), "prl_head_logprob: workspace too small");
-  if (M > kBlockM && !sampled_ids && !sampled_logprobs && g_use_2cta && !g_tiled_weights) {
-    // many tokens, statistics only (learner forward, reference-logprob scoring): CTA-pair kernel, token-per-thread
+  if (M > kBlockM && !sampled_ids && !sampled_logprobs && !g_tiled_weights) {
+    // many tokens, statistics only (learner forward, reference-logprob scoring): 128 x 256 tiles, token-per-thread
     // epilogue (csrc/gemm_tn.cu)
     return head_logprob_tn(W, W_lo, X, M, V, K, temperature, targets, logprob_target, entropy, lse, workspace,
                            (cudaStream_t)stream_);

@@ -1,21 +1,19 @@
-// CTA-pair tcgen05 GEMM for the compute-bound shapes of the learner (hot path 2) and of prefill / scoring:
+// wgmma GEMM for the compute-bound shapes of the learner (hot path 2) and of prefill / scoring:
 //
-//   C[M, N] (=|+=) A[M, K] * B[N, K]^T  (+ bias[N]) (+ residual[M, N])     bf16 operands, fp32 accumulation in TMEM
+//   C[M, N] (=|+=) A[M, K] * B[N, K]^T  (+ bias[N]) (+ residual[M, N])     bf16 operands, fp32 accumulation
 //
 // replaces the cuBLAS GEMMs behind the HF Qwen2 forward/backward that rl_step drives
 // (pipelinerl/finetune/rl/__init__.py:190-207 forward; finetune_loop.py:716-725 backward): with K-major ("TN")
 // operands the same kernel serves
 //   forward   Y  = X  * W^T            A = X [T, in],        B = W [out, in]
-//   dgrad     dX = dY * W              A = dY [T, out],      B = W^T [in, out]     (transposed weight copy)
-//   wgrad     dW += dY^T * X           A = dY^T [out, T],    B = X^T [in, T]       (fp32 accumulate epilogue)
+//   dgrad     dX = dY * W              A = dY [T, out],      B = W [out, in] read as stored (MN-major B)
+//   wgrad     dW += dY^T * X           A = dY^T (MN-major),  B = X^T (MN-major)     (fp32 accumulate epilogue)
 //
-// One (2,1,1) cluster owns a 256 x 256 output tile: CTA r stages A rows [128 r, 128 r + 128) and B rows
-// [128 r, 128 r + 128) of the tile per 64-wide k-block (TMA, SWIZZLE_128B, 6-stage ring, 32 KB/stage/CTA), the
-// leader issues tcgen05.mma.cta_group::2 (UMMA 256x256x16), and CTA r's TMEM receives its 128 A-rows x all 256
-// columns, so every epilogue thread owns ONE output row and writes contiguous row segments (16-byte stores).
-// The kernel is persistent: each cluster walks tiles in an L2-friendly order (8 row-tiles x all column tiles per
-// super-group), and the 512 TMEM columns hold TWO accumulators so that the epilogue of tile i overlaps the
-// mainloop of tile i + 1.
+// One CTA owns a 128 x 256 output tile: a TMA producer warp stages A rows [128) and B rows [256) of the tile per 64-wide
+// k-block (SWIZZLE_128B, 4-stage ring, 48 KB/stage), two consumer warpgroups each run wgmma m64n256k16 on 64 of the A
+// rows with fp32 accumulators in registers.  After the mainloop the accumulators go through the drained ring to shared
+// memory so that every epilogue thread owns ONE output row and half of its columns, and writes contiguous row segments
+// (16-byte stores).  CTAs walk the tiles in an L2-friendly order (8 row-tiles x all column tiles per super-group).
 //
 // Tensor-core bound: flops = 2 M N K; algorithmic bytes = 2 (M K + N K) + out bytes.
 #include "prl_common.cuh"
@@ -24,13 +22,18 @@
 namespace prl {
 namespace {
 
-constexpr int kTile = 256;      // output tile edge per cluster
-constexpr int kHalf = 128;      // operand rows staged per CTA
+constexpr int kTileM = 128;     // output rows per CTA (two wgmma M = 64 halves)
+constexpr int kTileN = 256;     // output columns per CTA (wgmma N)
+constexpr int kHalf = 128;      // operand rows per TMA box
 constexpr int kBK = 64;         // bf16 per k-block row = one 128-B swizzle atom
-constexpr int kStages = 6;
-constexpr int kStageBytes = 2 * kHalf * kBK * 2;  // 32 KB
+constexpr int kStages = 4;
+constexpr int kABytes = kTileM * kBK * 2;          // 16 KB
+constexpr int kStageBytes = kABytes + kTileN * kBK * 2;  // 48 KB
 constexpr int kMnChunkBytes = 64 * kBK * 2;        // one 64(MN) x 64(k) box of an MN-major operand: 8 KB
-constexpr int kThreadsTN = 192;
+constexpr int kEpiLd = kTileN + 4;                 // fp32 accumulator tile [128][260] in the drained ring
+static_assert(kTileM * kEpiLd * 4 <= kStages * kStageBytes, "epilogue tile must fit in the ring");
+constexpr int kSmemTN = kStages * kStageBytes + 1024 + 8 * (2 * kStages) + 16;
+constexpr int kThreadsTN = 288;
 constexpr int kGroupM = 8;      // row tiles per raster super-group
 
 struct TnParams {
@@ -55,7 +58,7 @@ struct TnParams {
   int swiglu_fp32;      // 1: SiLU(gate) * up of the fp32 ACCUMULATORS (the sampler's rounding points, decode_ops.cu silu_mul_kernel)
   __nv_bfloat16* act;      // [M, ld_act]
   int64_t ld_act;
-  // head epilogue (kHead): logits never leave TMEM/registers
+  // head epilogue (kHead): logits never leave the SM
   const int64_t* targets;  // [M] or NULL
   float4* head_part;       // [n_tiles, M]: (max, sum exp, sum exp*z, target logit or -inf) of one 256-column vocabulary tile
   // head BACKWARD epilogue (kHead, dz != NULL): the logits tile is turned into d loss / d logits in registers and only its
@@ -83,8 +86,9 @@ __device__ __forceinline__ void tile_coords(int t, const TnParams& p, int& tm, i
   tn = r / rows;
 }
 
-template <bool kHead>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreadsTN, 1)
+// Warp roles (288 threads): warps 0..7 = two consumer warpgroups, warp 8 = TMA producer.
+template <bool kHead, int kAmn, int kBmn>
+__global__ void __launch_bounds__(kThreadsTN, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                const __grid_constant__ CUtensorMap tm_b2, TnParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -92,123 +96,117 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
   const uint32_t bar_base = smem_base + (uint32_t)(kStages * kStageBytes);
   auto full_bar = [&](int s) { return bar_base + 8u * (uint32_t)s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (uint32_t)(kStages + s); };
-  auto acc_full_bar = [&](int a) { return bar_base + 8u * (uint32_t)(2 * kStages + a); };       // MMA -> epilogue
-  auto acc_empty_bar = [&](int a) { return bar_base + 8u * (uint32_t)(2 * kStages + 2 + a); };  // epilogue -> MMA
-  const uint32_t tmem_slot = bar_base + 8u * (uint32_t)(2 * kStages + 4);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = ptx::cluster_ctarank();
-  const int n_clusters = (int)gridDim.x >> 1;
-  const int cluster = (int)blockIdx.x >> 1;
-  const int total_tiles = p.m_tiles * p.n_tiles;
+  int tm, tn;
+  tile_coords((int)blockIdx.x, p, tm, tn);
 
-  if (threadIdx.x == 0) {
+  if (threadIdx.x == 256) {
     for (int s = 0; s < kStages; ++s) {
-      ptx::mbar_init(full_bar(s), 2);   // leader expect_tx + peer's remote arrive (rank 0's copy is the one used)
-      ptx::mbar_init(empty_bar(s), 1);  // multicast tcgen05.commit
-    }
-    for (int a = 0; a < 2; ++a) {
-      ptx::mbar_init(acc_full_bar(a), 1);   // multicast tcgen05.commit
-      ptx::mbar_init(acc_empty_bar(a), 2);  // one elected epilogue thread of EACH CTA (rank 0's copy is the one used)
+      ptx::mbar_init(full_bar(s), 1);
+      ptx::mbar_init(empty_bar(s), 2);   // one elected thread of each consumer warpgroup
     }
     ptx::fence_barrier_init();
     ptx::fence_proxy_async();
     ptx::prefetch_tensormap(&tm_a);
     ptx::prefetch_tensormap(&tm_b);
   }
-  ptx::cluster_sync();
-  if (warp == 1) {
-    ptx::tmem_alloc_2sm(tmem_slot, 512);
-    ptx::tmem_relinquish_2sm();
-  }
-  ptx::tc_fence_before_sync();
-  ptx::cluster_sync();
-  ptx::tc_fence_after_sync();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
+  __syncthreads();
 
-  if (warp == 0) {
-    // ===== TMA producer (both CTAs) =====
+  if (warp == 8) {
+    // ===== TMA producer =====
     if (lane == 0) {
-      int it = 0;
-      for (int t = cluster; t < total_tiles; t += n_clusters) {
-        int tm, tn;
-        tile_coords(t, p, tm, tn);
-        const int a_row = tm * kTile + (int)rank * kHalf;
-        const int b_row = p.swiglu_I ? tn * kHalf + (int)rank * (int)p.swiglu_I : tn * kTile + (int)rank * kHalf;
-        for (int kb = 0; kb < p.kblocks; ++kb, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (uint32_t)((it / kStages) & 1);
-          ptx::mbar_wait(empty_bar(s), ph ^ 1u);
-          if (rank == 0) ptx::mbar_arrive_expect_tx(full_bar(s), 2u * (uint32_t)kStageBytes);
-          else ptx::mbar_arrive_remote(full_bar(s), 0);
-          const uint32_t a_dst = smem_base + (uint32_t)(s * kStageBytes);
-          const uint32_t b_dst = a_dst + kHalf * kBK * 2;
-          const bool second = kb >= p.k_wrap;                 // hi + lo operand streams (K-major operands only)
-          const int kk = (second ? kb - p.k_wrap : kb) * kBK;
-          const CUtensorMap* tb = second ? &tm_b2 : &tm_b;
-          if (!p.a_mn) {
-            ptx::tma_load_2d_2sm(a_dst, &tm_a, kk, a_row, full_bar(s), ptx::kEvictNormal);
-          } else {  // two 64(MN) x 64(k) boxes: inner coordinate = MN index, outer = k
-            ptx::tma_load_2d_2sm(a_dst, &tm_a, a_row, kk, full_bar(s), ptx::kEvictNormal);
-            ptx::tma_load_2d_2sm(a_dst + kMnChunkBytes, &tm_a, a_row + 64, kk, full_bar(s), ptx::kEvictNormal);
-          }
-          if (!p.b_mn) {
-            ptx::tma_load_2d_2sm(b_dst, tb, kk, b_row, full_bar(s), ptx::kEvictNormal);
-          } else {
-            ptx::tma_load_2d_2sm(b_dst, tb, b_row, kk, full_bar(s), ptx::kEvictNormal);
-            ptx::tma_load_2d_2sm(b_dst + kMnChunkBytes, tb, b_row + 64, kk, full_bar(s), ptx::kEvictNormal);
-          }
+      const int a_row = tm * kTileM;
+      // B rows of the tile in two 128-row halves; SwiGLU: the gate rows and the up rows of the SAME 128 features
+      const int b_row0 = p.swiglu_I ? tn * kHalf : tn * kTileN;
+      const int b_row1 = p.swiglu_I ? (int)p.swiglu_I + tn * kHalf : tn * kTileN + kHalf;
+      for (int kb = 0; kb < p.kblocks; ++kb) {
+        const int s = kb % kStages;
+        ptx::mbar_wait(empty_bar(s), (uint32_t)(((kb / kStages) & 1) ^ 1));
+        ptx::mbar_arrive_expect_tx(full_bar(s), (uint32_t)kStageBytes);
+        const uint32_t a_dst = smem_base + (uint32_t)(s * kStageBytes);
+        const uint32_t b_dst = a_dst + kABytes;
+        const bool second = kb >= p.k_wrap;                 // hi + lo operand streams (K-major operands only)
+        const int kk = (second ? kb - p.k_wrap : kb) * kBK;
+        const CUtensorMap* tb = second ? &tm_b2 : &tm_b;
+        if (!kAmn) {
+          ptx::tma_load_2d(a_dst, &tm_a, kk, a_row, full_bar(s), ptx::kEvictNormal);
+        } else {  // two 64(MN) x 64(k) boxes: inner coordinate = MN index, outer = k
+          ptx::tma_load_2d(a_dst, &tm_a, a_row, kk, full_bar(s), ptx::kEvictNormal);
+          ptx::tma_load_2d(a_dst + kMnChunkBytes, &tm_a, a_row + 64, kk, full_bar(s), ptx::kEvictNormal);
+        }
+        if (!kBmn) {
+          ptx::tma_load_2d(b_dst, tb, kk, b_row0, full_bar(s), ptx::kEvictNormal);
+          ptx::tma_load_2d(b_dst + kHalf * kBK * 2, tb, kk, b_row1, full_bar(s), ptx::kEvictNormal);
+        } else {
+          ptx::tma_load_2d(b_dst, tb, b_row0, kk, full_bar(s), ptx::kEvictNormal);
+          ptx::tma_load_2d(b_dst + kMnChunkBytes, tb, b_row0 + 64, kk, full_bar(s), ptx::kEvictNormal);
+          ptx::tma_load_2d(b_dst + 2 * kMnChunkBytes, tb, b_row1, kk, full_bar(s), ptx::kEvictNormal);
+          ptx::tma_load_2d(b_dst + 3 * kMnChunkBytes, tb, b_row1 + 64, kk, full_bar(s), ptx::kEvictNormal);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (leader CTA only) =====
-    if (lane == 0 && rank == 0) {
-      const uint32_t idesc = ptx::make_idesc_bf16_f32(kTile, kTile) | ((uint32_t)p.a_mn << 15) | ((uint32_t)p.b_mn << 16);
-      const uint64_t a_step = p.a_mn ? 128u : 2u, b_step = p.b_mn ? 128u : 2u;  // K += 16 in (addr >> 4) units
-      int it = 0, local = 0;
-      for (int t = cluster; t < total_tiles; t += n_clusters, ++local) {
-        const int acc = local & 1;
-        const uint32_t acc_ph = (uint32_t)((local >> 1) & 1);
-        ptx::mbar_wait(acc_empty_bar(acc), acc_ph ^ 1u);  // both CTAs' epilogues have drained this accumulator
-        ptx::tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * kTile);
-        for (int kb = 0; kb < p.kblocks; ++kb, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (uint32_t)((it / kStages) & 1);
-          ptx::mbar_wait(full_bar(s), ph);
-          ptx::tc_fence_after_sync();
-          const uint32_t a_addr = smem_base + (uint32_t)(s * kStageBytes);
-          const uint32_t b_addr = a_addr + kHalf * kBK * 2;
-          const uint64_t a_desc = p.a_mn ? ptx::make_mnmajor_sw128_desc(a_addr, kMnChunkBytes) : ptx::make_kmajor_sw128_desc(a_addr);
-          const uint64_t b_desc = p.b_mn ? ptx::make_mnmajor_sw128_desc(b_addr, kMnChunkBytes) : ptx::make_kmajor_sw128_desc(b_addr);
+    return;
+  }
+
+  // ===== consumers: warpgroup wg = tile rows [64 wg, 64 wg + 64) x all 256 columns =====
+  const int wg = warp >> 2;
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  constexpr uint64_t a_step = kAmn ? 128u : 2u, b_step = kBmn ? 128u : 2u;  // K += 16 in (addr >> 4) units
+  float acc[kTileN / 2];
 #pragma unroll
-          for (int k = 0; k < kBK / 16; ++k)
-            ptx::mma_bf16_ss_2sm(d_tmem, a_desc + a_step * (uint64_t)k, b_desc + b_step * (uint64_t)k, idesc,
-                                 (kb > 0 || k > 0) ? 1u : 0u);
-          ptx::tc_commit_2sm(empty_bar(s), 3);
-        }
-        ptx::tc_commit_2sm(acc_full_bar(acc), 3);
-      }
+  for (int e = 0; e < kTileN / 2; ++e) acc[e] = 0.f;
+  for (int kb = 0; kb < p.kblocks; ++kb) {
+    const int s = kb % kStages;
+    ptx::mbar_wait(full_bar(s), (uint32_t)((kb / kStages) & 1));
+    const uint32_t a_addr = smem_base + (uint32_t)(s * kStageBytes) + (uint32_t)(wg * kMnChunkBytes);
+    const uint32_t b_addr = smem_base + (uint32_t)(s * kStageBytes) + kABytes;
+    const uint64_t a_desc = kAmn ? ptx::make_mnmajor_sw128_desc(a_addr, kMnChunkBytes) : ptx::make_kmajor_sw128_desc(a_addr);
+    const uint64_t b_desc = kBmn ? ptx::make_mnmajor_sw128_desc(b_addr, kMnChunkBytes) : ptx::make_kmajor_sw128_desc(b_addr);
+    ptx::fence_acc(acc);
+    ptx::wg_fence();
+#pragma unroll
+    for (int k = 0; k < kBK / 16; ++k)
+      ptx::wgmma_ss<kAmn, kBmn>(acc, a_desc + a_step * (uint64_t)k, b_desc + b_step * (uint64_t)k, 1u);
+    ptx::wg_commit();
+    ptx::wg_wait<1>();                       // the previous stage's wgmmas are done: release that slot
+    if (kb > 0 && wg_leader) ptx::mbar_arrive(empty_bar((kb - 1) % kStages));
+  }
+  ptx::wg_wait<0>();
+  ptx::fence_acc(acc);
+
+  // ---- accumulators -> fp32 tile [128 rows][kEpiLd] in the drained ring ----
+  asm volatile("bar.sync 1, 256;" ::: "memory");   // both warpgroups are past their last shared-memory operand read
+  float* stile = reinterpret_cast<float*>(smem_raw + (smem_base - ptx::smem_u32(smem_raw)));
+  {
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < kTileN / 8; ++j) {
+      const int c = 8 * j + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(stile + r0 * kEpiLd + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(stile + (r0 + 8) * kEpiLd + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
-    __syncwarp();
-  } else {
-    // ===== epilogue (both CTAs): thread = one output row, 256 columns in 32-column chunks =====
-    const int q = warp & 3;
-    int local = 0;
-    for (int t = cluster; t < total_tiles; t += n_clusters, ++local) {
-      int tm, tn;
-      tile_coords(t, p, tm, tn);
-      const int acc = local & 1;
-      const uint32_t acc_ph = (uint32_t)((local >> 1) & 1);
-      ptx::mbar_wait(acc_full_bar(acc), acc_ph);
-      ptx::tc_fence_after_sync();
-      const int64_t row = (int64_t)tm * kTile + (int64_t)rank * kHalf + q * 32 + lane;
-      const int64_t col0 = (int64_t)tn * kTile;
+  }
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+
+  // ===== epilogue: thread = one output row, columns [128 h, 128 h + 128) in 32-column chunks =====
+  {
+    const int lrow = threadIdx.x & 127;
+    const int h = threadIdx.x >> 7;
+    const float* srow = stile + lrow * kEpiLd;
+    auto ld32 = [&](int c, uint32_t (&r)[32]) {
+#pragma unroll
+      for (int j = 0; j < 32; j += 4) {
+        const float4 f = *reinterpret_cast<const float4*>(srow + c + j);
+        r[j] = __float_as_uint(f.x); r[j + 1] = __float_as_uint(f.y); r[j + 2] = __float_as_uint(f.z); r[j + 3] = __float_as_uint(f.w);
+      }
+    };
+    {
+      const int64_t row = (int64_t)tm * kTileM + lrow;
+      const int64_t col0 = (int64_t)tn * kTileN + h * kHalf;
       const bool row_ok = row < p.M;
       if constexpr (kHead) {
-        // thread = one token; online softmax statistics over this tile's 256 vocabulary columns, all thread-local
+        // thread = one token; online softmax statistics over 128 vocabulary columns of the tile, all thread-local
         constexpr float kLog2e = 1.4426950408889634f;
         const int64_t tgt = (p.targets && row_ok) ? p.targets[row] : -1;
         if (p.dz != nullptr) {
@@ -218,12 +216,11 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
           const float ge = (p.bwd_g_ent && row_ok) ? p.bwd_g_ent[row] : 0.f;
           const float H = (p.bwd_g_ent && p.bwd_ent && row_ok) ? p.bwd_ent[row] : 0.f;
 #pragma unroll 1
-          for (int c0 = 0; c0 < kTile; c0 += 32) {
+          for (int c0 = 0; c0 < kHalf; c0 += 32) {
             if (col0 + c0 >= p.N) break;
-            uint32_t r[32];
-            ptx::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * kTile + c0), r);
-            ptx::tmem_ld_wait();
             if (!row_ok) continue;
+            uint32_t r[32];
+            ld32(h * kHalf + c0, r);
             const int64_t col = col0 + c0;
             const int n_ok = (int)((p.N - col) < 32 ? (p.N - col) : 32);
             __nv_bfloat16* dst = p.dz + row * p.ld_dz + col;
@@ -255,11 +252,10 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
         } else {
         float m = -INFINITY, ssum = 0.f, usum = 0.f, zt = -INFINITY;
 #pragma unroll 1
-        for (int c0 = 0; c0 < kTile; c0 += 32) {
+        for (int c0 = 0; c0 < kHalf; c0 += 32) {
           if (col0 + c0 >= p.N) break;
           uint32_t r[32];
-          ptx::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * kTile + c0), r);
-          ptx::tmem_ld_wait();
+          ld32(h * kHalf + c0, r);
           const int64_t col = col0 + c0;
           const int n_ok = (int)((p.N - col) < 32 ? (p.N - col) : 32);
           float z[32];
@@ -288,18 +284,18 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
               if (rel == (uint64_t)j) zt = z[j];
           }
         }
-        if (row_ok) p.head_part[(int64_t)tn * p.M + row] = make_float4(m, ssum, usum, zt);
+        if (row_ok) p.head_part[(int64_t)(2 * tn + h) * p.M + row] = make_float4(m, ssum, usum, zt);
         }   // forward statistics
       } else if (p.swiglu_I) {
-        // columns 0..127 of the accumulator = gate, 128..255 = up of features [tn * 128, tn * 128 + 128)
+        // columns 0..127 of the tile = gate, 128..255 = up of features [tn * 128, tn * 128 + 128); thread half h takes
+        // features [64 h, 64 h + 64)
         const int64_t f0 = (int64_t)tn * kHalf;
 #pragma unroll 1
-        for (int c0 = 0; c0 < kHalf; c0 += 32) {
-          uint32_t rg[32], ru[32];
-          ptx::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * kTile + c0), rg);
-          ptx::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * kTile + kHalf + c0), ru);
-          ptx::tmem_ld_wait();
+        for (int c0 = h * 64; c0 < h * 64 + 64; c0 += 32) {
           if (!row_ok) continue;
+          uint32_t rg[32], ru[32];
+          ld32(c0, rg);
+          ld32(kHalf + c0, ru);
           __nv_bfloat16* ap = p.act + row * p.ld_act + f0 + c0;
           __nv_bfloat16* gp = p.C ? reinterpret_cast<__nv_bfloat16*>(p.C) + row * p.ldc + f0 + c0 : nullptr;
 #pragma unroll
@@ -332,12 +328,11 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
         }
       } else {
 #pragma unroll 1
-      for (int c0 = 0; c0 < kTile; c0 += 32) {
-        if (col0 + c0 >= p.N) break;  // uniform across the CTA
-        uint32_t r[32];
-        ptx::tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * kTile + c0), r);
-        ptx::tmem_ld_wait();
+      for (int c0 = 0; c0 < kHalf; c0 += 32) {
+        if (col0 + c0 >= p.N) break;
         if (!row_ok) continue;
+        uint32_t r[32];
+        ld32(h * kHalf + c0, r);
         const int64_t col = col0 + c0;
         const bool full = (col + 32 <= p.N);
         float v[32];
@@ -432,21 +427,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
         }
       }
       }  // !kHead
-      // this CTA's four epilogue warps are done with the accumulator -> tell the leader's MMA warp
-      ptx::tc_fence_before_sync();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (threadIdx.x == 64) {
-        if (rank == 0) ptx::mbar_arrive(acc_empty_bar(acc));
-        else ptx::mbar_arrive_remote(acc_empty_bar(acc), 0);
-      }
     }
-  }
-
-  ptx::tc_fence_before_sync();
-  ptx::cluster_sync();
-  if (warp == 1) {
-    ptx::tc_fence_after_sync();
-    ptx::tmem_dealloc_2sm(tmem_base, 512);
   }
 }
 
@@ -527,6 +508,27 @@ __global__ void __launch_bounds__(256) transpose_bf16_kernel(const __nv_bfloat16
   }
 }
 
+// one CTA per 128 x 256 output tile; the operand majorness is a compile-time property of the wgmma instruction
+template <bool kHead, int kAmn, int kBmn>
+int launch_tn_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tb2, const TnParams& p, cudaStream_t stream) {
+  static SmemAttr smem_attr = {};
+  PRL_CUDA(ensure_smem(gemm_tn_kernel<kHead, kAmn, kBmn>, kSmemTN, smem_attr));
+  const int64_t tiles = (int64_t)p.m_tiles * p.n_tiles;
+  PRL_CHECK_ARG(tiles < (1ll << 31), "prl_gemm_tn: too many output tiles");
+  gemm_tn_kernel<kHead, kAmn, kBmn><<<dim3((unsigned)tiles), dim3(kThreadsTN), (size_t)kSmemTN, stream>>>(ta, tb, tb2, p);
+  PRL_LAUNCH_CHECK();
+  return PRL_OK;
+}
+
+int launch_tn(bool head, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tb2, const TnParams& p,
+              cudaStream_t stream) {
+  if (head) return launch_tn_t<true, 0, 0>(ta, tb, tb2, p, stream);
+  if (p.a_mn && p.b_mn) return launch_tn_t<false, 1, 1>(ta, tb, tb2, p, stream);
+  if (p.a_mn) return launch_tn_t<false, 1, 0>(ta, tb, tb2, p, stream);
+  if (p.b_mn) return launch_tn_t<false, 0, 1>(ta, tb, tb2, p, stream);
+  return launch_tn_t<false, 0, 0>(ta, tb, tb2, p, stream);
+}
+
 }  // namespace
 }  // namespace prl
 
@@ -555,8 +557,8 @@ extern "C" int prl_gemm_ex(const void* A, int64_t lda, int32_t a_mn_major, const
   p.M = M; p.N = N; p.K = K;
   p.kblocks = (int)((K + kBK - 1) / kBK);
   p.k_wrap = p.kblocks;
-  p.m_tiles = (int)((M + kTile - 1) / kTile);
-  p.n_tiles = (int)((N + kTile - 1) / kTile);
+  p.m_tiles = (int)((M + kTileM - 1) / kTileM);
+  p.n_tiles = (int)((N + kTileN - 1) / kTileN);
   p.C = C; p.ldc = ldc; p.c_f32 = c_is_f32; p.accumulate = accumulate;
   p.bias = (const __nv_bfloat16*)bias;
   p.residual = (const __nv_bfloat16*)residual;
@@ -571,14 +573,8 @@ extern "C" int prl_gemm_ex(const void* A, int64_t lda, int32_t a_mn_major, const
   rc = b_mn_major ? make_tmap_2d_bf16(&tb, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb * 2, 64, kBK)
                   : make_tmap_2d_bf16(&tb, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, kBK, kHalf);
   if (rc) return rc;
-  const int smem = kStages * kStageBytes + 1024 + 8 * (2 * kStages + 4) + 16;
-  static SmemAttr smem_attr = {};
-  PRL_CUDA(ensure_smem(gemm_tn_kernel<false>, smem, smem_attr));
-  const int64_t tiles = (int64_t)p.m_tiles * p.n_tiles;
-  int clusters = num_sms() / 2;
-  if (tiles < clusters) clusters = (int)tiles;
-  gemm_tn_kernel<false><<<dim3((unsigned)(2 * clusters)), dim3(kThreadsTN), (size_t)smem, (cudaStream_t)stream_>>>(ta, tb, tb, p);
-  PRL_LAUNCH_CHECK();
+  rc = launch_tn(false, ta, tb, tb, p, (cudaStream_t)stream_);
+  if (rc) return rc;
   return PRL_OK;
 }
 
@@ -595,8 +591,8 @@ extern "C" int prl_gemm_dgrad_swiglu(const void* dY, int64_t ldy, const void* W_
   p.M = M; p.N = I; p.K = H;
   p.kblocks = (int)((H + kBK - 1) / kBK);
   p.k_wrap = p.kblocks;
-  p.m_tiles = (int)((M + kTile - 1) / kTile);
-  p.n_tiles = (int)((I + kTile - 1) / kTile);
+  p.m_tiles = (int)((M + kTileM - 1) / kTileM);
+  p.n_tiles = (int)((I + kTileN - 1) / kTileN);
   p.alpha = 1.f;
   p.b_mn = 1;
   p.bwd_gu = (const __nv_bfloat16*)gate_up; p.dgu = (__nv_bfloat16*)d_gate_up; p.ld_gu = ld_gu;
@@ -605,14 +601,8 @@ extern "C" int prl_gemm_dgrad_swiglu(const void* dY, int64_t ldy, const void* W_
   if (rc) return rc;
   rc = make_tmap_2d_bf16(&tb, W_down, (uint64_t)I, (uint64_t)H, (uint64_t)ldw * 2, 64, kBK);
   if (rc) return rc;
-  const int smem = kStages * kStageBytes + 1024 + 8 * (2 * kStages + 4) + 16;
-  static SmemAttr smem_attr = {};
-  PRL_CUDA(ensure_smem(gemm_tn_kernel<false>, smem, smem_attr));
-  const int64_t tiles = (int64_t)p.m_tiles * p.n_tiles;
-  int clusters = num_sms() / 2;
-  if (tiles < clusters) clusters = (int)tiles;
-  gemm_tn_kernel<false><<<dim3((unsigned)(2 * clusters)), dim3(kThreadsTN), (size_t)smem, (cudaStream_t)stream_>>>(ta, tb, tb, p);
-  PRL_LAUNCH_CHECK();
+  rc = launch_tn(false, ta, tb, tb, p, (cudaStream_t)stream_);
+  if (rc) return rc;
   return PRL_OK;
 }
 
@@ -646,7 +636,7 @@ static int gemm_swiglu_impl(const void* X, int64_t ldx, const void* W, int64_t l
   p.M = M; p.N = 2 * I; p.K = K;
   p.kblocks = (int)((K + kBK - 1) / kBK);
   p.k_wrap = p.kblocks;
-  p.m_tiles = (int)((M + kTile - 1) / kTile);
+  p.m_tiles = (int)((M + kTileM - 1) / kTileM);
   p.n_tiles = (int)(I / kHalf);
   p.C = gate_up; p.ldc = ld_gu; p.alpha = 1.f;
   p.swiglu_I = I; p.swiglu_fp32 = fp32_act; p.act = (__nv_bfloat16*)act; p.ld_act = ld_act;
@@ -655,20 +645,15 @@ static int gemm_swiglu_impl(const void* X, int64_t ldx, const void* W, int64_t l
   if (rc) return rc;
   rc = make_tmap_2d_bf16(&tb, W, (uint64_t)K, (uint64_t)(2 * I), (uint64_t)ldw * 2, kBK, kHalf);
   if (rc) return rc;
-  const int smem = kStages * kStageBytes + 1024 + 8 * (2 * kStages + 4) + 16;
-  static SmemAttr smem_attr = {};
-  PRL_CUDA(ensure_smem(gemm_tn_kernel<false>, smem, smem_attr));
-  const int64_t tiles = (int64_t)p.m_tiles * p.n_tiles;
-  int clusters = num_sms() / 2;
-  if (tiles < clusters) clusters = (int)tiles;
-  gemm_tn_kernel<false><<<dim3((unsigned)(2 * clusters)), dim3(kThreadsTN), (size_t)smem, (cudaStream_t)stream_>>>(ta, tb, tb, p);
-  PRL_LAUNCH_CHECK();
+  rc = launch_tn(false, ta, tb, tb, p, (cudaStream_t)stream_);
+  if (rc) return rc;
   return PRL_OK;
 }
 
 namespace prl {
 // fused output head for many tokens (M > 128): logprob of the target, entropy and logsumexp of softmax(X W^T / T)
-// without storing logits.  Called by prl_head_logprob (gemm_tc.cu).  workspace: ceil(V/256) * M float4.
+// without storing logits.  Called by prl_head_logprob (gemm_tc.cu).  workspace: 2 ceil(V/256) * M float4 (one per
+// 128-column half of a tile).
 int head_logprob_tn(const void* W, const void* W_lo, const void* X, int64_t M, int64_t V, int64_t K, float temperature,
                     const int64_t* targets, float* logprob_target, float* entropy, float* lse, void* workspace,
                     cudaStream_t stream) {
@@ -676,9 +661,9 @@ int head_logprob_tn(const void* W, const void* W_lo, const void* X, int64_t M, i
   p.M = M; p.N = V; p.K = K;
   p.kblocks = (int)((K + kBK - 1) / kBK);
   p.k_wrap = p.kblocks;
-  if (W_lo) p.kblocks *= 2;          // logits = X W_hi^T + X W_lo^T accumulated in the same TMEM tile
-  p.m_tiles = (int)((M + kTile - 1) / kTile);
-  p.n_tiles = (int)((V + kTile - 1) / kTile);
+  if (W_lo) p.kblocks *= 2;          // logits = X W_hi^T + X W_lo^T accumulated in the same registers
+  p.m_tiles = (int)((M + kTileM - 1) / kTileM);
+  p.n_tiles = (int)((V + kTileN - 1) / kTileN);
   p.alpha = 1.f / temperature;
   p.targets = targets;
   p.head_part = (float4*)workspace;
@@ -689,15 +674,9 @@ int head_logprob_tn(const void* W, const void* W_lo, const void* X, int64_t M, i
   if (rc) return rc;
   rc = make_tmap_2d_bf16(&tb2, W_lo ? W_lo : W, (uint64_t)K, (uint64_t)V, (uint64_t)K * 2, kBK, kHalf);
   if (rc) return rc;
-  const int smem = kStages * kStageBytes + 1024 + 8 * (2 * kStages + 4) + 16;
-  static SmemAttr smem_attr = {};
-  PRL_CUDA(ensure_smem(gemm_tn_kernel<true>, smem, smem_attr));
-  const int64_t tiles = (int64_t)p.m_tiles * p.n_tiles;
-  int clusters = num_sms() / 2;
-  if (tiles < clusters) clusters = (int)tiles;
-  gemm_tn_kernel<true><<<dim3((unsigned)(2 * clusters)), dim3(kThreadsTN), (size_t)smem, stream>>>(ta, tb, tb2, p);
-  PRL_LAUNCH_CHECK();
-  head_tn_combine_kernel<<<(unsigned)((M + 3) / 4), 128, 0, stream>>>((const float4*)workspace, p.n_tiles, M,
+  rc = launch_tn(true, ta, tb, tb2, p, stream);
+  if (rc) return rc;
+  head_tn_combine_kernel<<<(unsigned)((M + 3) / 4), 128, 0, stream>>>((const float4*)workspace, 2 * p.n_tiles, M,
                                                                       targets ? 1 : 0, logprob_target, entropy, lse);
   PRL_LAUNCH_CHECK();
   return PRL_OK;
@@ -705,7 +684,7 @@ int head_logprob_tn(const void* W, const void* W_lo, const void* X, int64_t M, i
 }  // namespace prl
 
 // Backward of the fused output head without materialised logits: dz[M, ld_dz] (bf16) = d loss / d logits for every row, from
-// ONE GEMM (X W_hi^T + X W_lo^T accumulated in TMEM, as the forward) whose epilogue applies
+// ONE GEMM (X W_hi^T + X W_lo^T accumulated together, as the forward) whose epilogue applies
 //   dz = inv_T * (g_lp * (onehot(target) - p) - g_ent * p * (log p + H)),   p = exp(z * inv_T - lse)
 // in registers (reference: autograd through logits/T -> log_softmax / entropy, rl/__init__.py:207-233).  dz is the operand of
 // the dX and dW GEMMs that follow; fp32 logits, fp32 d logits and the cast pass never exist.
@@ -724,8 +703,8 @@ extern "C" int prl_head_dlogits(const void* W, const void* W_lo, const void* X, 
   p.kblocks = (int)((K + kBK - 1) / kBK);
   p.k_wrap = p.kblocks;
   if (W_lo) p.kblocks *= 2;
-  p.m_tiles = (int)((M + kTile - 1) / kTile);
-  p.n_tiles = (int)((V + kTile - 1) / kTile);
+  p.m_tiles = (int)((M + kTileM - 1) / kTileM);
+  p.n_tiles = (int)((V + kTileN - 1) / kTileN);
   p.alpha = 1.f / temperature;
   p.targets = targets;
   p.dz = (__nv_bfloat16*)dz_bf16; p.ld_dz = ld_dz;
@@ -737,14 +716,8 @@ extern "C" int prl_head_dlogits(const void* W, const void* W_lo, const void* X, 
   if (rc) return rc;
   rc = make_tmap_2d_bf16(&tb2, W_lo ? W_lo : W, (uint64_t)K, (uint64_t)V, (uint64_t)K * 2, kBK, kHalf);
   if (rc) return rc;
-  const int smem = kStages * kStageBytes + 1024 + 8 * (2 * kStages + 4) + 16;
-  static SmemAttr smem_attr = {};
-  PRL_CUDA(ensure_smem(gemm_tn_kernel<true>, smem, smem_attr));
-  const int64_t tiles = (int64_t)p.m_tiles * p.n_tiles;
-  int clusters = num_sms() / 2;
-  if (tiles < clusters) clusters = (int)tiles;
-  gemm_tn_kernel<true><<<dim3((unsigned)(2 * clusters)), dim3(kThreadsTN), (size_t)smem, (cudaStream_t)stream_>>>(ta, tb, tb2, p);
-  PRL_LAUNCH_CHECK();
+  rc = launch_tn(true, ta, tb, tb2, p, (cudaStream_t)stream_);
+  if (rc) return rc;
   return PRL_OK;
 }
 

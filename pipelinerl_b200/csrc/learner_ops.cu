@@ -11,7 +11,7 @@ namespace {
 
 constexpr int kRowThreads = 256;
 constexpr int kMaxVec = 4;          // 8-element vectors per thread -> rows of up to 8192 elements
-constexpr int kPartialBlocks = 592; // 4 per SM: grid of the persistent row kernels = rows of the partial workspace
+constexpr int kPartialBlocks = 528; // 4 per SM: grid of the persistent row kernels = rows of the partial workspace
 
 struct Vec8 { float v[8]; };
 
@@ -361,7 +361,7 @@ extern "C" int prl_rope_inplace(void* x, int64_t ld, int64_t T, int32_t n_heads,
 extern "C" int prl_silu_mul_fwd(const void* gate_up, int64_t T, int64_t I, void* act, prl_stream_t stream) {
   PRL_CHECK_ARG(gate_up && act && T >= 1 && I >= 8 && I % 8 == 0, "prl_silu_mul_fwd: bad argument (I %% 8 == 0)");
   const int64_t blocks = (T * (I / 8) + 255) / 256;
-  silu_mul_fwd_kernel<<<(unsigned)(blocks < 148 * 16 ? blocks : 148 * 16), 256, 0, (cudaStream_t)stream>>>(
+  silu_mul_fwd_kernel<<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)gate_up, T, (int)I, (__nv_bfloat16*)act);
   PRL_LAUNCH_CHECK();
   return PRL_OK;
@@ -371,7 +371,7 @@ extern "C" int prl_silu_mul_bwd(const void* gate_up, const void* dact, int64_t T
                                 prl_stream_t stream) {
   PRL_CHECK_ARG(gate_up && dact && dgate_up && T >= 1 && I >= 8 && I % 8 == 0, "prl_silu_mul_bwd: bad argument");
   const int64_t blocks = (T * (I / 8) + 255) / 256;
-  silu_mul_bwd_kernel<<<(unsigned)(blocks < 148 * 16 ? blocks : 148 * 16), 256, 0, (cudaStream_t)stream>>>(
+  silu_mul_bwd_kernel<<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)gate_up, (const __nv_bfloat16*)dact, T, (int)I, (__nv_bfloat16*)dgate_up);
   PRL_LAUNCH_CHECK();
   return PRL_OK;

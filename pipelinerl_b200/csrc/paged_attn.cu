@@ -14,8 +14,7 @@
 //     tensor cores are used for issue efficiency, not throughput), online softmax in
 //     fp32 (exp2 domain), ldmatrix with the matching XOR swizzle (conflict-free);
 //   * per-split (m, l, O) partials are merged either by a small combine kernel (default) or by whichever split
-//     CTA of the (sequence, kv head) finishes last (arrival ticket; prl_attn_set_fused_combine) — A/B measured in
-//     profiles/r1_ablation*.jsonl.
+//     CTA of the (sequence, kv head) finishes last (arrival ticket; prl_attn_set_fused_combine).
 // KV cache layout (bf16): row = (((layer*2 + kv) * n_pages + page) * n_kv + kvh) * 64 + slot,
 // 128 contiguous d per row — written by qkv_rope_cache_kernel (decode_ops.cu).
 #include "prl_common.cuh"

@@ -313,7 +313,7 @@ __global__ void __launch_bounds__(kThreads) pg_loss_kernel(prl_pg_batch b, prl_p
   }
 }
 
-constexpr int kMaxBlocks = 148 * 8;
+constexpr int kMaxBlocks = 132 * 8;
 
 }  // namespace
 }  // namespace prl

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libprl.so (sm_100a only).
+// Shared host/device helpers for libprl.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -7,8 +7,8 @@
 #include <stdarg.h>
 #include "../../include/prl.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libprl is written for sm_100a only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libprl is written for sm_90a only"
 #endif
 
 namespace prl {

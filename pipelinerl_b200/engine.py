@@ -55,7 +55,7 @@ class DecodeEngine:
                  device: torch.device | str = "cuda:0", use_cuda_graph: bool = True, prefill_chunk: int = 1024,
                  prefix_sharing: bool = True, fused_head: bool = False):
         if cfg.head_dim != 128:
-            raise ValueError("the sm_100a attention kernel is built for head_dim 128")
+            raise ValueError("the sm_90a attention kernel is built for head_dim 128")
         self.cfg, self.arena = cfg, arena
         self.lib = _lib.load()
         self.dev = torch.device(device)
@@ -71,11 +71,11 @@ class DecodeEngine:
         self.use_graph = use_cuda_graph
         # fused_head: lm_head + sampling + logprob capture in one GEMM epilogue (no logits in HBM).  For the 64-row
         # decode step the logits round trip is only 78 MB and the fused epilogue cannot live in the step's CUDA graph
-        # (its RNG arguments change per step), so the unfused path measured 1.5 % faster (profiles/r1_ablation_b.jsonl);
+        # (its RNG arguments change per step), so the step keeps the unfused path;
         # the fused kernel is what scoring / the trainer's forward use, where the logits would be 608 KB per token.
         self.fused_head = fused_head
-        self.l2_prefetch_bytes = 0          # cross-kernel L2 prefetch budget per site; measured to HURT (+0.19 ms/step,
-                                            # profiles/r1_ablation.jsonl: HBM is already saturated), so off
+        self.l2_prefetch_bytes = 0          # cross-kernel L2 prefetch budget per site; off: the step is HBM-bound, prefetching
+                                            # only moves the same bytes earlier
         self._skip: set[str] = set()        # timing ablations only (tools/step_ablation.py)
         # SiLU(gate) * up in the gate_up GEMM's epilogue (prl_gemm_swiglu_decode); PRL_FUSE_SWIGLU=0 keeps the two-kernel pair
         self.fuse_swiglu = os.environ.get("PRL_FUSE_SWIGLU", "1") != "0"
@@ -128,7 +128,7 @@ class DecodeEngine:
         self._graphs: dict[int, torch.cuda.CUDAGraph] = {}
         # ---- chunked prefill + prefix sharing (GRPO attempts share their prompt) ----
         self.prefill_chunk = int(prefill_chunk)
-        self.prefill_attn_tc = os.environ.get("PRL_PREFILL_ATTN", "tc") != "mma"   # tcgen05 (default) | mma.sync kernel
+        self.prefill_attn_tc = os.environ.get("PRL_PREFILL_ATTN", "tc") != "mma"   # wgmma (default) | mma.sync kernel
         self.prefix_sharing = prefix_sharing
         self.page_ref = [0] * self.n_pages
         self._prefill_queue: list[Request] = []
@@ -393,7 +393,7 @@ class DecodeEngine:
                                          a.ptr("layers.0.input_layernorm.weight"), cfg.rms_eps, n, H, cfg.vocab_size,
                                          h.data_ptr(), x.data_ptr(), st))
         max_q = max(k for _, _, k in segs)
-        big = n > 128   # compute-bound chunk: persistent CTA-pair GEMM; o/down accumulate straight into the fp32 residual
+        big = n > 128   # compute-bound chunk: 128x256-tile wgmma GEMM; o/down accumulate straight into the fp32 residual
 
         def gemm(w_name, src, N, K, dst, accumulate=False):
             if big:
@@ -415,7 +415,7 @@ class DecodeEngine:
                                               self.inv_freq.data_ptr(), pf["q"].data_ptr(), self.kv_cache.data_ptr(),
                                               self.n_pages, l, PAGE_SIZE, None, 0, st))
             seq = pf["seq"]
-            if self.prefill_attn_tc:   # tcgen05 path (csrc/attn_tc.cu)
+            if self.prefill_attn_tc:   # wgmma path (csrc/attn_tc.cu)
                 _lib.check(lib.prl_paged_attn_prefill_tc(pf["q"].data_ptr(), n, self.kv_cache.data_ptr(), self.n_pages,
                                                          cfg.num_layers, l, self.block_table.data_ptr(), self.max_blocks,
                                                          seq[0].data_ptr(), seq[1].data_ptr(), seq[2].data_ptr(),

@@ -3,14 +3,14 @@
 `fused_head_logprobs(hidden, weight, targets, temperature)` returns, per token, the log-probability of its
 target and the exact entropy of softmax(logits / T) — what rl_step derives from full-vocabulary fp32 logits at
 pipelinerl/finetune/rl/__init__.py:207-233 (608 KB/token for Qwen2.5; 10 GB for a 16 K-token micro-batch, plus a
-/T copy and a detached copy).  Forward: ONE tcgen05 GEMM whose epilogue reduces each 128-row vocabulary tile in
-TMEM to (max, sum exp, sum exp*z, target logit) — `prl_head_logprob`, csrc/gemm_tc.cu.  Backward: logits are
-recomputed chunk by chunk (tcgen05 GEMM into a bounded scratch), turned into d logits in place
+/T copy and a detached copy).  Forward: ONE wgmma GEMM whose epilogue reduces each 128-row vocabulary tile on
+chip to (max, sum exp, sum exp*z, target logit) — `prl_head_logprob`, csrc/gemm_tc.cu.  Backward: logits are
+recomputed chunk by chunk (wgmma GEMM into a bounded scratch), turned into d logits in place
 (csrc/logprob_tail.cu) and contracted with two library GEMMs (torch.mm -> cuBLAS: plain GEMMs), so peak extra
 memory is one chunk, never T x V.
 
 The fp32 master weight is split into a bf16 value and a bf16 residual (W = hi + lo): both streams feed the same
-TMEM accumulator, which reproduces the reference's fp32 lm_head (finetune/checkpoints.py:44-105) to ~2^-17.
+fp32 accumulator, which reproduces the reference's fp32 lm_head (finetune/checkpoints.py:44-105) to ~2^-17.
 """
 from __future__ import annotations
 
@@ -72,7 +72,7 @@ class _FusedHead(torch.autograd.Function):
             n = min(C, M - r0)
             xs = x[r0:r0 + n]
             logits, dlogits = logits_buf[:n], dlogits_buf[:n]
-            # recompute this chunk's logits with the same tcgen05 kernel and operands as the forward
+            # recompute this chunk's logits with the same wgmma kernel and operands as the forward
             _lib.check(lib.prl_gemm_bf16_splitk(hi.data_ptr(), lo.data_ptr() if lo is not None else None, xs.data_ptr(),
                                                 n, V, K, 1, logits.data_ptr(), st))
             _lib.check(lib.prl_logprob_rows_bwd(logits.data_ptr(), n, V, V, tg[r0:r0 + n].data_ptr(), ctx.temperature,

@@ -1,4 +1,4 @@
-"""RL step of the trainer, on the sm_100a kernels of libprl.so.
+"""RL step of the trainer, on the sm_90a kernels of libprl.so.
 
 Keeps the reference's operator boundary (pipelinerl/finetune/rl/__init__.py):
 

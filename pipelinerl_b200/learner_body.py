@@ -8,12 +8,12 @@ conf/finetune/base.yaml:47-50 checkpointing).  Here there is no autograd inside 
             -> RMSNorm -> gate_up GEMM -> SiLU*up -> down GEMM(+residual); only each layer's INPUT is kept
   backward  per layer (reverse): recompute the MLP half (and the attention half where it was not kept), then dgrad
             GEMMs that read the weights as stored and wgrad GEMMs that read both activations as stored (MN-major
-            UMMA operands: no transposed copies) and ACCUMULATE IN FP32 straight into the optimizer's gradient
+            wgmma operands: no transposed copies) and ACCUMULATE IN FP32 straight into the optimizer's gradient
             arena (no .grad tensors, no autograd accumulation kernels, no per-parameter allocation)
 
-Every GEMM is `prl_gemm_ex` (csrc/gemm_tn.cu, persistent CTA-pair tcgen05 kernel).  The row-wise pieces (RMSNorm, RoPE, SiLU*up, bias / gain reductions, embedding
+Every GEMM is `prl_gemm_ex` (csrc/gemm_tn.cu, wgmma kernel with 128x256 tiles).  The row-wise pieces (RMSNorm, RoPE, SiLU*up, bias / gain reductions, embedding
 scatter) are the kernels of csrc/learner_ops.cu.  Attention (the flash-attn varlen call of the reference) is the
-tcgen05 forward of csrc/attn_tc.cu and the two-kernel deterministic backward of csrc/attn_train.cu.
+wgmma forward of csrc/attn_tc.cu and the two-kernel deterministic backward of csrc/attn_bwd.cu.
 """
 from __future__ import annotations
 
@@ -237,7 +237,7 @@ class NativeBody:
     def refresh(self) -> None:
         """Hook called after every optimizer step.  Nothing to rebuild: dgrad reads the weights as stored."""
 
-    # ---- attention: q, k roped; block-diagonal causal over the packed segments (csrc/attn_tc.cu, attn_train.cu) ----
+    # ---- attention: q, k roped; block-diagonal causal over the packed segments (csrc/attn_tc.cu, attn_bwd.cu) ----
     def _segments(self, bounds, dev):
         key = tuple(bounds)
         if self._seg_cache is None or self._seg_cache[0] != key or self._seg_cache[1].device != dev:

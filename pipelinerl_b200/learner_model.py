@@ -1,7 +1,7 @@
 """Learner-side Qwen2 modules whose parameters live in the fused arena layout (model.py).
 
-`NativeQwen2` (bottom of this file) is the B200 learner: its body is learner_body.NativeBody — hand-scheduled forward /
-backward on the persistent CTA-pair tcgen05 GEMM and the row kernels of csrc/learner_ops.cu, fp32 gradient accumulation
+`NativeQwen2` (bottom of this file) is the native learner: its body is learner_body.NativeBody — hand-scheduled forward /
+backward on the wgmma GEMM and the row kernels of csrc/learner_ops.cu, fp32 gradient accumulation
 in the optimizer arena, fused head without logits.  It is what `run_training`, tools/train_bench.py and
 tools/pipeline_bench.py use.
 
@@ -65,7 +65,7 @@ class TorchQwen2(torch.nn.Module):
         return torch.cat([x1 * cs - x2 * sn, x2 * cs + x1 * sn], dim=-1)
 
     def forward_logprobs(self, batch, temperature: float):
-        """rl_step's fast path: (new_logprobs [B, L-1], entropy [B, L-1]) through the fused tcgen05 head — the
+        """rl_step's fast path: (new_logprobs [B, L-1], entropy [B, L-1]) through the fused wgmma head — the
         [L, V] logits are never materialised (finetune/fused_head.py)."""
         from .finetune.fused_head import fused_head_logprobs
         hidden = self.hidden_states(batch.input_ids, batch.position_ids if batch.is_packed else None)
@@ -121,8 +121,8 @@ class TorchQwen2(torch.nn.Module):
 
 
 class _NativeHead(torch.autograd.Function):
-    """Final projection + log-softmax statistics of the native learner.  Forward: one tcgen05 GEMM whose epilogue
-    reduces logits in TMEM (prl_head_logprob).  Backward: per chunk of rows, the same GEMM again with an epilogue that turns
+    """Final projection + log-softmax statistics of the native learner.  Forward: one wgmma GEMM whose epilogue
+    reduces logits on chip (prl_head_logprob).  Backward: per chunk of rows, the same GEMM again with an epilogue that turns
     the logits tile into d logits in registers and stores it as bf16 (prl_head_dlogits), then dX = dZ W and dW += dZ^T X
     (prl_gemm_ex, operands read as stored), the latter accumulated in fp32 in the optimizer's gradient arena."""
 
@@ -198,7 +198,7 @@ class _NativeHead(torch.autograd.Function):
 
 
 class NativeQwen2(torch.nn.Module):
-    """Learner model whose body is learner_body.NativeBody (hand-scheduled tcgen05 GEMMs + row kernels, fp32
+    """Learner model whose body is learner_body.NativeBody (hand-scheduled wgmma GEMMs + row kernels, fp32
     gradient accumulation in the optimizer arena).  bf16 parameters in the fused arena order; must be bound to a
     FusedAdamW(grad_dtype=torch.float32) with `bind(optimizer)` before the first step."""
 

@@ -65,6 +65,12 @@ class ModelConfig:
                            num_q_heads=28, num_kv_heads=4, **kw)
 
     @staticmethod
+    def qwen2_5_1_5b(**kw) -> "ModelConfig":
+        """Qwen2.5-1.5B's shapes (its input and output embeddings are stored untied here)."""
+        return ModelConfig(vocab_size=151936, hidden_size=1536, intermediate_size=8960, num_layers=28,
+                           num_q_heads=12, num_kv_heads=2, **kw)
+
+    @staticmethod
     def qwen2_5_32b(**kw) -> "ModelConfig":
         return ModelConfig(vocab_size=152064, hidden_size=5120, intermediate_size=27648, num_layers=64,
                            num_q_heads=40, num_kv_heads=8, **kw)

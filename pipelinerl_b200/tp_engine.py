@@ -149,7 +149,8 @@ class TPDecodeEngine(DecodeEngine):
         tiles = (self.cfg.hidden_size + 127) // 128
         kb_o = (self.cfg.q_size + 63) // 64
         kb_d = (self.cfg.intermediate_size + 63) // 64
-        s = max(1, -(-148 // tiles))
+        sms = torch.cuda.get_device_properties(self.dev).multi_processor_count
+        s = max(1, -(-sms // tiles))
         s = max(1, min(s, kb_o // 4, kb_d // 4))
         self.split_k["o"] = self.split_k["down"] = s
 

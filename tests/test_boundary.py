@@ -38,11 +38,11 @@ def test_version_and_error_string(built_lib):
     assert built_lib.prl_pg_workspace_bytes(16) > 0 and built_lib.prl_adamw_workspace_bytes() > 0
 
 
-def test_sm100a_cubin_present():
+def test_sm90a_cubin_present():
     import subprocess
     from pipelinerl_b200 import _lib
     out = subprocess.run(["cuobjdump", "--list-elf", str(_lib.lib_path())], capture_output=True, text=True).stdout
-    assert "sm_100a" in out, out
+    assert "sm_90a" in out, out
 
 
 def test_product_never_imports_oracle():

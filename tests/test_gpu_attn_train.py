@@ -1,4 +1,4 @@
-"""Learner attention on sm_100a (csrc/attn_tc.cu forward, csrc/attn_train.cu backward) against an fp32 reference.
+"""Learner attention on sm_90a (csrc/attn_tc.cu forward, csrc/attn_bwd.cu backward) against an fp32 reference.
 
 The op: block-diagonal causal attention over one packed row -- what the reference gets from flash-attn varlen
 through HF when `position_ids` restart per packed sample (pipelinerl/finetune/rl/__init__.py:204,
@@ -52,8 +52,9 @@ def _reference(qkv, d_out, bounds, n_q, n_kv):
 
 
 def _run(dev, n_q, n_kv, lens, seed=0, pad_cols=0, fwd_gen=2, bwd_gen=None):
-    """fwd_gen / bwd_gen: 1 = operands through shared memory, 2 = P / dS handed to the tensor core through TMEM (default);
-    bwd_gen 3 = 2 + Q / dO resident in TMEM, 4 = 16 decoupled softmax warps"""
+    """fwd_gen: 1 = O rescaled at every step, 2 = only when a row's maximum grew by more than 2^8 (default);
+    bwd_gen: how P / dS reach the tensor core -- 1 = shared memory in both kernels, 2 = registers (default),
+    3 = registers in dK/dV and shared memory in dQ, 4 = shared memory in dK/dV and registers in dQ"""
     from pipelinerl_b200 import _lib
     o = _ops()
     bwd_gen = fwd_gen if bwd_gen is None else bwd_gen
@@ -92,7 +93,7 @@ def _run(dev, n_q, n_kv, lens, seed=0, pad_cols=0, fwd_gen=2, bwd_gen=None):
         scale = max(want_d[:, a:b].abs().max().item(), 1e-3)      # a single-token segment has dq = dk = 0 exactly
         res[name] = (dqkv[:, a:b].float() - want_d[:, a:b]).abs().max().item() / scale
     _lib.check(o.lib.prl_attn_set_fwd_generation(2))
-    _lib.check(o.lib.prl_attn_set_bwd_generation(4))
+    _lib.check(o.lib.prl_attn_set_bwd_generation(2))
     print(f"[attn_train fwd gen{fwd_gen} bwd gen{bwd_gen}] n_q={n_q} n_kv={n_kv} lens={lens if len(lens) < 8 else str(lens[:6]) + '...'}: " +
           " ".join(f"{k}={v:.2e}" for k, v in res.items()))
     assert res["out"] <= 2 ** -7, res

@@ -1,4 +1,4 @@
-"""tcgen05 weight-streaming GEMM (csrc/gemm_tc.cu) against a plain fp32 torch matmul of the same bf16
+"""wgmma weight-streaming GEMM (csrc/gemm_tc.cu) against a plain fp32 torch matmul of the same bf16
 operands.  Tolerance: fp32 accumulation of bf16 products -> 1e-4 relative to the row scale."""
 import pytest
 import torch
@@ -23,7 +23,7 @@ def run_gemm(W, X, W_lo=None, split_k=0):
 SHAPES = [
     (1, 128, 64, 1), (16, 256, 128, 2), (37, 300, 200, 1), (64, 4608, 3584, 0), (64, 3584, 18944, 0),
     (33, 1152, 512, 3), (128, 640, 1024, 2), (200, 384, 256, 1), (300, 256, 192, 1), (64, 37888, 3584, 0),
-    # M > 128 runs the CTA-pair (tcgen05 cta_group::2) kernel: ragged token / feature / k tails, split-K, many k-blocks
+    # M > 128: 256-token tiles with ragged token / feature / k tails, split-K, many k-blocks
     (129, 128, 64, 1), (513, 777, 200, 1), (256, 512, 4096, 2), (1024, 4608, 3584, 1), (700, 1000, 1288, 3),
 ]
 
@@ -39,23 +39,6 @@ def test_gemm_matches_fp32_matmul(cuda_device, M, N, K, split_k):
     want = X.float() @ W.float().t()
     scale = want.abs().max().item()
     assert (got - want).abs().max().item() <= 2e-4 * scale + 1e-6
-
-
-def test_cta_pair_kernel_agrees_with_single_cta(cuda_device):
-    """Same operands through both M>128 kernels: fp32 accumulation order per element is identical (k ascending),
-    so the two tiles must agree BITWISE."""
-    from pipelinerl_b200 import _lib
-    lib = _lib.load()
-    g = torch.Generator().manual_seed(11)
-    X = torch.randn(600, 1536, generator=g).to(torch.bfloat16).to(cuda_device)
-    W = (torch.randn(1000, 1536, generator=g) * 0.05).to(torch.bfloat16).to(cuda_device)
-    try:
-        _lib.check(lib.prl_gemm_set_cta_pair(0))
-        single = run_gemm(W, X, split_k=2)
-    finally:
-        _lib.check(lib.prl_gemm_set_cta_pair(1))
-    pair = run_gemm(W, X, split_k=2)
-    assert torch.equal(single, pair)
 
 
 def test_gemm_hi_lo_is_fp32_equivalent(cuda_device):
@@ -132,7 +115,7 @@ def test_fused_head_logprob_capture(cuda_device, M, V, K):
 @pytest.mark.parametrize("M,V,K,with_targets", [(129, 640, 256, True), (1000, 4096 + 77, 512, True),
                                                 (2048, 152064, 128, True), (300, 1000, 264, False)])
 def test_fused_head_many_tokens_statistics_only(cuda_device, M, V, K, with_targets):
-    """M > 128 without sampling outputs runs the CTA-pair kernel with the token-per-thread epilogue (gemm_tn.cu)."""
+    """M > 128 without sampling outputs runs the 128 x 256-tile kernel with the token-per-thread epilogue (gemm_tn.cu)."""
     from pipelinerl_b200 import _lib
     lib = _lib.load()
     g = torch.Generator().manual_seed(V + M)
@@ -158,8 +141,8 @@ def test_fused_head_many_tokens_statistics_only(cuda_device, M, V, K, with_targe
 
 @pytest.mark.parametrize("B,I,K", [(4, 128, 256), (16, 1152, 896), (64, 18944, 3584), (100, 256, 512), (33, 192, 64)])
 def test_token_step_swiglu_epilogue_is_bit_identical_to_gemm_plus_silu(cuda_device, B, I, K):
-    """prl_gemm_swiglu_decode (the CTA's 128 weight rows = 64 gate rows + the 64 up rows of the same features; the up half
-    crosses to the gate half's threads through shared memory) == prl_gemm_bf16_splitk(split_k = 1) + prl_silu_mul, bit for bit."""
+    """prl_gemm_swiglu_decode (the CTA's 128 weight rows = 64 gate rows + the 64 up rows of the same features, both halves
+    read back from the shared-memory accumulator tile) == prl_gemm_bf16_splitk(split_k = 1) + prl_silu_mul, bit for bit."""
     from pipelinerl_b200 import _lib
     lib = _lib.load()
     dev = cuda_device

@@ -1,4 +1,4 @@
-"""CTA-pair persistent tcgen05 GEMM of the learner body (csrc/gemm_tn.cu) against fp32 torch matmuls of the
+"""wgmma GEMM of the learner body (csrc/gemm_tn.cu) against fp32 torch matmuls of the
 same bf16 operands.  Tolerance: fp32 accumulation of bf16 products (1e-4 of the output scale) plus one bf16
 rounding (2^-8 relative) where the output is bf16."""
 import pytest
@@ -176,7 +176,7 @@ def test_gemm_swiglu_f32_is_bit_identical_to_fp32_gemm_plus_sampler_silu(cuda_de
 @pytest.mark.parametrize("M,V,K,with_lo,with_ent", [(300, 1031, 256, True, True), (2048, 4096, 512, True, False),
                                                      (130, 777, 128, False, True), (1, 520, 64, True, True)])
 def test_head_dlogits_without_materialised_logits(cuda_device, M, V, K, with_lo, with_ent):
-    """prl_head_dlogits: the head GEMM (hi + lo weight streams in one TMEM accumulation) with the backward of
+    """prl_head_dlogits: the head GEMM (hi + lo weight streams in one accumulation) with the backward of
     log-softmax / entropy in its epilogue, bf16 d logits out.  Against fp32 torch autograd through logits / T ->
     log_softmax -> (target logprob, entropy) on the same bf16 inputs, and the statistics of prl_head_logprob as inputs."""
     from pipelinerl_b200 import _lib

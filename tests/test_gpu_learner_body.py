@@ -13,8 +13,8 @@ from tests.helpers import tiny_cfg, tiny_weights
 
 pytestmark = pytest.mark.gpu
 
-# end-to-end bounds (bf16 activations against fp32 references) = 1.5 x what a B200 measured; the tests print the measured values
-# measured: hidden rel L2 0.0061 / 0.0068, max |dlogprob| 0.0118 / 0.0192, worst gradient rel L2 0.0086 / 0.0104 (gqa2 / gqa7)
+# end-to-end bounds (bf16 activations against fp32 references) with about 1.5 x headroom; the tests print the measured values
+# measured on an H100: hidden rel L2 0.0061 / 0.0068, max |dlogprob| 0.0118 / 0.0152, worst gradient rel L2 0.0087 / 0.0104 (gqa2 / gqa7)
 BODY_BOUNDS = {"hidden": 1.02e-2, "logprob": 2.9e-2, "grad": 1.56e-2}
 # measured vs the reference's rl_step on HF fp32: loss rel 3.6e-6 / 4.0e-3, gradient-norm rel 0.0013 / 0.0015, sampled gradients 0.0131 / 0.0117
 HF_STEP_BOUNDS = {"loss": 6e-3, "grad_norm": 2.3e-3, "grad_samples": 2e-2}
@@ -259,7 +259,7 @@ def test_full_size_layer_recompute_modes_agree(cuda_device):
 def test_native_learner_vs_reference_rl_step_on_hf(cuda_device, kind):
     """Hot path 2 end to end against the REFERENCE: tests/golden/learner_step_*.npz holds the reference's rl_step run on
     HF Qwen2ForCausalLM (fp32, CPU) for one packed micro-batch.  Here: our rl_step on NativeQwen2 (bf16 activations,
-    tcgen05 GEMMs, fused head, fused PG loss) -> backward -> fp32 gradient arena.  Tolerances are the bf16 noise floor of
+    wgmma GEMMs, fused head, fused PG loss) -> backward -> fp32 gradient arena.  Tolerances are the bf16 noise floor of
     a transformer with bf16 activations: loss 2e-2 relative, logprobs 3e-2 absolute, every gradient tensor 3e-2 in
     norm and 5e-2 relative L2 on the stored elements."""
     import json

@@ -179,7 +179,7 @@ def test_large_row_properties(cuda_device):
 
 
 def test_rl_step_fused_head_matches_logits_path(cuda_device):
-    """rl_step through a model exposing forward_logprobs (tcgen05 fused head, no [T, V] logits) == rl_step through
+    """rl_step through a model exposing forward_logprobs (wgmma fused head, no [T, V] logits) == rl_step through
     the same model's materialised logits: loss, stats and every parameter gradient."""
     from pipelinerl_b200.finetune.rl import RLConfig, rl_step
     from pipelinerl_b200.learner_model import TorchQwen2

@@ -1,6 +1,6 @@
 """Whole loop on one GPU with a tiny model: plugin rollouts through the in-process engine -> preprocess ->
 packed micro-batches (cut at the optimizer-step boundary) -> rl_step on the NATIVE learner (learner_model.NativeQwen2:
-tcgen05 GEMMs, tcgen05 attention forward / backward, fused head, fp32 gradient arena) -> FusedAdamW -> in-flight weight
+wgmma GEMMs, wgmma attention forward / backward, fused head, fp32 gradient arena) -> FusedAdamW -> in-flight weight
 push -> sampler flip."""
 import asyncio
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Learner attention forward / backward (csrc/attn_tc.cu, csrc/attn_train.cu) on Qwen2.5-7B's head geometry, timed
+"""Learner attention forward / backward (csrc/attn_tc.cu, csrc/attn_bwd.cu) on Qwen2.5-7B's head geometry, timed
 with CUDA events next to the library kernel it replaced (torch SDPA -> cuDNN flash) on the same inputs.
 
     python tools/attn_bench.py [--tokens 16384] [--segments 1] [--reps 10]
@@ -39,12 +39,9 @@ def main():
     ap.add_argument("--n-kv", type=int, default=4)
     ap.add_argument("--no-library", action="store_true")
     ap.add_argument("--ours-only", action="store_true", help="one forward + one backward of our kernels, nothing else (ncu)")
-    ap.add_argument("--tmem", action="store_true", help="TMEM read bandwidth microbenchmark")
-    ap.add_argument("--phases", action="store_true", help="per-phase cycle counts of one CTA of the generation-2 forward")
-    ap.add_argument("--mma", action="store_true", help="tcgen05.mma issue-rate / hand-off microbenchmark only")
     ap.add_argument("--profile", action="store_true", help="per-kernel device time (torch profiler)")
-    ap.add_argument("--fwd-gen", type=int, default=0, help="forward generation for --profile / --ours-only")
-    ap.add_argument("--bwd-gen", type=int, default=0, help="backward generation for --profile / --ours-only (0 = library default)")
+    ap.add_argument("--fwd-gen", type=int, default=0, help="forward generation (0 = library default)")
+    ap.add_argument("--bwd-gen", type=int, default=0, help="backward generation (0 = library default)")
     a = ap.parse_args()
     dev = torch.device("cuda:0")
     o = Ops()
@@ -56,103 +53,23 @@ def main():
     d_out = torch.randn(T, n_q * D, generator=g, device=dev).to(torch.bfloat16)
     st = torch.arange(0, T, L, dtype=torch.int32, device=dev)
     ln = torch.tensor(lens, dtype=torch.int32, device=dev)
-    from pipelinerl_b200 import _lib as _l0
-    if a.bwd_gen:
-        _l0.check(o.lib.prl_attn_set_bwd_generation(a.bwd_gen))
     if a.fwd_gen:
-        _l0.check(o.lib.prl_attn_set_fwd_generation(a.fwd_gen))
-    if a.mma:
-        lib = _l0.load()
-        o2 = torch.zeros(2, dtype=torch.int64, device=dev)
-        names = {0: "ss_128x128", 1: "ss_128x64", 2: "ss_128x256", 3: "ss_b_mnmajor_128x128", 4: "ts_128x128",
-                 5: "ts_b_mnmajor_128x128", 6: "ts_128x256", 7: "ts_128x64", 8: "ss_128x128_two_accumulators",
-                 9: "ss_batch_then_ts_mnmajor_batch", 10: "handoff_round_trip"}
-        res = {"bench": "tcgen05_mma_issue", "cycles_per_umma": {}}
-        for mode, nm in names.items():
-            for _ in range(2):
-                _l0.check(lib.prl_debug_mma_bench(mode, 2000, o2.data_ptr(), _l0.stream_ptr()))
-                torch.cuda.synchronize()
-            res["cycles_per_umma"][nm] = round(int(o2[0]) / int(o2[1]), 1)
-        print(json.dumps(res), flush=True)
-        return
-    if a.phases:
-        lib = _l0.load()
-        _l0.check(o.lib.prl_attn_set_fwd_generation(2))
-        t20 = torch.zeros(20, dtype=torch.int64, device=dev)
-        o.attn_fwd(qkv, st, ln, L, n_q, n_kv, D)
-        _l0.check(lib.prl_attn_debug_timing(t20.data_ptr()))
-        o.attn_fwd(qkv, st, ln, L, n_q, n_kv, D)
-        torch.cuda.synchronize()
-        _l0.check(lib.prl_attn_debug_timing(None))
-        v = t20.tolist()
-        steps = max(v[19], 1)
-        names = ["wait_S", "tmem_ld", "mask_max", "wait_O_rescale", "exp_pack_st", "barrier_arrive"]
-        res = {"bench": "attn_fwd_v2_phases", "steps_of_cta0": v[19],
-               "group0_cycles_per_own_step": {n: round(v[i] / ((steps + 1) // 2), 1) for i, n in enumerate(names)},
-               "group1_cycles_per_own_step": {n: round(v[8 + i] / max(steps // 2, 1), 1) for i, n in enumerate(names)},
-               "mma_warp_cycles_per_step": {"wait_P": round(v[16] / steps, 1), "wait_V": round(v[17] / steps, 1),
-                                            "total": round(v[18] / steps, 1)}}
-        print(json.dumps(res), flush=True)
-        out, lse = o.attn_fwd(qkv, st, ln, L, n_q, n_kv, D)
-        _l0.check(o.lib.prl_attn_set_bwd_generation(4))
-        o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D)
-        t16 = torch.zeros(16, dtype=torch.int64, device=dev)
-        _l0.check(lib.prl_attn_debug_bwd_timing(t16.data_ptr()))
-        o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D)
-        torch.cuda.synchronize()
-        _l0.check(lib.prl_attn_debug_bwd_timing(None))
-        v = t16.tolist()
-        steps = max(v[13], 1)
-        print(json.dumps({"bench": "attn_bwd_dq4_phases", "steps_of_cta0": v[13],
-                          "softmax_warp_cycles_per_step": {n: round(v[i] / steps, 1) for i, n in
-                                                           enumerate(["wait_S", "ld_exp", "wait_dP", "ld_dS_st_arrive"])},
-                          "mma_warp_cycles_per_step": {n: round(v[8 + i] / steps, 1) for i, n in
-                                                       enumerate(["wait_K", "wait_S_drained", "wait_dS", "wait_V", "total"])}}), flush=True)
-        t16.zero_()
-        _l0.check(lib.prl_attn_debug_bwd_timing_dkdv(t16.data_ptr()))
-        o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D)
-        torch.cuda.synchronize()
-        _l0.check(lib.prl_attn_debug_bwd_timing(None))
-        v = t16.tolist()
-        steps = max(v[13], 1)
-        own = max((steps + 1) // 2, 1)
-        print(json.dumps({"bench": "attn_bwd_dkdv4_phases", "sub_steps_of_cta0": v[13],
-                          "softmax_warp_cycles_per_own_step": {n: round(v[i] / own, 1) for i, n in
-                                                               enumerate(["group_barrier", "wait_ST_dPT", "ld_exp", "dS_st_arrive"])},
-                          "mma_warp_cycles_per_sub_step": {"wait_Q_dO": round(v[8] / steps, 1), "wait_PT_dST": round(v[9] / steps, 1),
-                                                           "total": round(v[12] / steps, 1)}}), flush=True)
-        return
+        o.lib.prl_attn_set_fwd_generation(a.fwd_gen)
+    if a.bwd_gen:
+        o.lib.prl_attn_set_bwd_generation(a.bwd_gen)
     if a.ours_only:
         for _ in range(2):
             out, lse = o.attn_fwd(qkv, st, ln, L, n_q, n_kv, D)
             o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D)
         torch.cuda.synchronize()
         return
-    from pipelinerl_b200 import _lib as _l
-    _l.check(o.lib.prl_attn_set_fwd_generation(1))
-    out1, _ = o.attn_fwd(qkv, st, ln, L, n_q, n_kv, D)
-    fwd1_ms = timed(lambda: o.attn_fwd(qkv, st, ln, L, n_q, n_kv, D), a.reps)
-    _l.check(o.lib.prl_attn_set_fwd_generation(2))
     out, lse = o.attn_fwd(qkv, st, ln, L, n_q, n_kv, D)
     fwd_ms = timed(lambda: o.attn_fwd(qkv, st, ln, L, n_q, n_kv, D), a.reps)
-    _l.check(o.lib.prl_attn_set_bwd_generation(1))
-    dq1 = o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D)
-    bwd1_ms = timed(lambda: o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D), a.reps)
-    _l.check(o.lib.prl_attn_set_bwd_generation(3))
-    dq3 = o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D)
-    bwd3_ms = timed(lambda: o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D), a.reps)
-    _l.check(o.lib.prl_attn_set_bwd_generation(2))
-    dq2 = o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D)
-    bwd2_ms = timed(lambda: o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D), a.reps)
-    _l.check(o.lib.prl_attn_set_bwd_generation(4))     # the default
-    dq4 = o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D)
+    o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D)
     bwd_ms = timed(lambda: o.attn_bwd(qkv, out, d_out, lse, st, ln, L, n_q, n_kv, D), a.reps)
     flops_fwd = a.segments * n_q * 4 * D * L * L / 2
     res = {"bench": "learner_attention", "tokens": T, "segments": a.segments, "n_q": n_q, "n_kv": n_kv,
-           "bwd_gen2_ms": round(bwd2_ms, 3), "bwd_gen4_vs_gen2_max_abs_diff": (dq4.float() - dq2.float()).abs().max().item(),
-           "bwd_gen3_ms": round(bwd3_ms, 3), "bwd_gen3_vs_gen2_max_abs_diff": (dq3.float() - dq2.float()).abs().max().item(),
-           "bwd_gen1_ms": round(bwd1_ms, 3), "bwd_gen1_vs_gen2_max_abs_diff": (dq1.float() - dq2.float()).abs().max().item(),
-           "fwd_gen1_ms": round(fwd1_ms, 3), "gen1_vs_gen2_max_abs_diff": (out1.float() - out.float()).abs().max().item(),
+           "fwd_gen": a.fwd_gen or "default", "bwd_gen": a.bwd_gen or "default",
            "ours": {"fwd_ms": round(fwd_ms, 3), "bwd_ms": round(bwd_ms, 3),
                     "fwd_TFLOPs": round(flops_fwd / fwd_ms / 1e9, 1), "bwd_TFLOPs": round(2.5 * flops_fwd / bwd_ms / 1e9, 1)}}
     if not a.no_library:
@@ -171,21 +88,7 @@ def main():
                                "bwd_TFLOPs": round(2.5 * flops_fwd / lb / 1e9, 1)}
         err = (y.transpose(1, 2).reshape(T, n_q * D).float() - out.float()).abs().max().item()
         res["max_abs_diff_vs_library_out"] = err
-    if a.tmem:
-        from pipelinerl_b200 import _lib
-        lib = _lib.load()
-        o3 = torch.zeros(3, dtype=torch.int64, device=dev)
-        res["tmem_read_bytes_per_clk_per_sm"] = {}
-        for w in (1, 2, 4, 8):
-            _lib.check(lib.prl_debug_tmem_read_bench(4096, w, o3.data_ptr(), _lib.stream_ptr()))
-            torch.cuda.synchronize()
-            cyc, nbytes = int(o3[0]), int(o3[1])
-            res["tmem_read_bytes_per_clk_per_sm"][f"{w}_warps"] = round(nbytes / cyc, 1)
     if a.profile:
-        if a.bwd_gen:
-            _l.check(o.lib.prl_attn_set_bwd_generation(a.bwd_gen))
-        if a.fwd_gen:
-            _l.check(o.lib.prl_attn_set_fwd_generation(a.fwd_gen))
         from torch.profiler import ProfilerActivity, profile as tprofile
         with tprofile(activities=[ProfilerActivity.CUDA]) as prof:
             for _ in range(3):

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Per-kernel timings at Qwen2.5-7B decode shapes (B=64) with an L2 flush between iterations.
-Used to choose tile / split-K / occupancy settings; summaries are copied to profiles/."""
+Used to choose tile / split-K / occupancy settings; it prints its summaries."""
 import json
 import sys
 from pathlib import Path

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Full rollouts through the plugin API on one B200 (BASELINE.json configs[1], sampler side, NOT a static-state microbench):
+"""Full rollouts through the plugin API on one GPU (BASELINE.json configs[1], sampler side, NOT a static-state microbench):
 
     generate_synthetic_rollout -> llm_async_generate -> EngineServer thread -> chunked prefill (1024-token chunks, the
     prompt shared by the 8 attempts of a GRPO group prefilled ONCE: page-hash prefix cache) -> decode with the context
@@ -69,7 +69,7 @@ def measure(problems=8, attempts=8, prompt_tokens=8192, max_tokens=8192, dev=Non
     kv_token_steps = sum(n * prompt_tokens + n * (n - 1) // 2 for n in n_out)
     alg_bytes = steps * (w_body + w_head) + kv_b * kv_token_steps
     peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text()) if (ROOT / "MEASURED_PEAKS.json").exists() else {}
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))   # H100 SXM data sheet when no measured peak is present
     out = {"bench": "rollout_full", "path": "generate_synthetic_rollout -> llm_async_generate -> EngineServer -> chunked "
            "prefill (prefix-shared per group) -> decode -> make_training_text", "model": "Qwen2.5-7B random-init",
            "rollouts": batch, "groups": problems, "attempts": attempts, "prompt_tokens": prompt_tokens,

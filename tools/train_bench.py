@@ -1,5 +1,5 @@
-"""Trainer step on random-init Qwen2.5-7B (hot path 2 end to end, one B200): rl_step (native body forward ->
-fused tcgen05 head -> PG loss) -> backward (native body, fp32 gradient accumulation) for `--micro` packed
+"""Trainer step on a random-init Qwen2.5 model (hot path 2 end to end, one GPU): rl_step (native body forward ->
+fused wgmma head -> PG loss) -> backward (native body, fp32 gradient accumulation) for `--micro` packed
 micro-batches of `--tokens` tokens, then the fused AdamW step and the refresh of the transposed weight copies.
 
 Prints one JSON line: tokens/s, seconds per optimizer step at the stated batch, model FLOPs utilisation against
@@ -64,12 +64,13 @@ def measure(model_name="7b", tokens=16384, samples_per_row=1, micro=2, steps=2, 
         log = log and rank == 0
     dev = dev or torch.device("cuda:0")
     torch.cuda.set_device(dev)
-    try:  # ~170 GB of the 192 GB are live at the peak: growable segments keep the caching allocator from fragmenting
+    try:  # most of the GPU's memory is live at the peak: growable segments keep the caching allocator from fragmenting
         torch.cuda.memory._set_allocator_settings("expandable_segments:True")
     except Exception:  # noqa: BLE001
         pass
     # fp32-equivalent lm_head (hi + lo bf16 operand streams), as the reference trains (finetune/checkpoints.py:44-105)
-    cfg = ModelConfig.qwen2_5_7b(fp32_head=fp32_head) if model_name == "7b" else ModelConfig.tiny(fp32_head=fp32_head)
+    configs = {"7b": ModelConfig.qwen2_5_7b, "1.5b": ModelConfig.qwen2_5_1_5b, "tiny": ModelConfig.tiny}
+    cfg = configs[model_name](fp32_head=fp32_head)
     if layers:
         from dataclasses import replace
         cfg = replace(cfg, num_layers=layers)
@@ -171,8 +172,8 @@ def measure(model_name="7b", tokens=16384, samples_per_row=1, micro=2, steps=2, 
     # model FLOPs: 6 N per token + causal attention (forward 1x + backward 2x); recompute is NOT counted
     model_flops = dp * micro * (6.0 * (body_params + head_params) * tokens + 3.0 * attn_fwd)
     peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text()) if (ROOT / "MEASURED_PEAKS.json").exists() else {}
-    peak = peaks.get("bf16_tflops_sustained", 1459.7)
-    out = {"bench": "trainer_step", "model": "Qwen2.5-7B" if model_name == "7b" else "tiny", "layers": c.num_layers,
+    peak = peaks.get("bf16_tflops_sustained", 989.0)   # H100 SXM data sheet, dense BF16 (not a measured rate)
+    out = {"bench": "trainer_step", "model": {"7b": "Qwen2.5-7B", "1.5b": "Qwen2.5-1.5B"}.get(model_name, model_name), "layers": c.num_layers,
            "tokens_per_micro_batch": tokens, "samples_per_micro_batch": samples_per_row, "micro_batches_per_step": micro,
            "samples_per_optimizer_step": n_samples_step, "ms_per_optimizer_step": round(ms, 2),
            "optimizer_steps_per_s": round(1000.0 / ms, 5), "trainer_tokens_per_s": round(total_tokens / ms * 1000.0, 1),
@@ -187,9 +188,9 @@ def measure(model_name="7b", tokens=16384, samples_per_row=1, micro=2, steps=2, 
            "peak_memory_GB": round(torch.cuda.max_memory_allocated() / 1e9, 1),
            "loss": rec[-1][4], "grad_norm": rec[-1][5], "grad_accumulation": "fp32 in the optimizer arena",
            "lm_head": "fp32-equivalent (bf16 hi + lo streams from the fp32 master)" if cfg.fp32_head else "bf16",
-           "attention": "prl_attn_varlen_fwd / prl_attn_varlen_bwd (tcgen05, csrc/attn_tc.cu + csrc/attn_train.cu)", "keep_attention_layers": model.body.keep_attention_layers,
+           "attention": "prl_attn_varlen_fwd / prl_attn_varlen_bwd (wgmma, csrc/attn_tc.cu + csrc/attn_bwd.cu)", "keep_attention_layers": model.body.keep_attention_layers,
            "keep_gate_up_layers": model.body.keep_gate_up_layers,
-           "gemm": "prl_gemm_ex (tcgen05 cta_group::2, MN-major dgrad/wgrad operands)"}
+           "gemm": "prl_gemm_ex (wgmma 128x256 tiles, MN-major dgrad/wgrad operands)"}
     del model, opt, batches
     import gc
     gc.collect()
@@ -199,7 +200,8 @@ def measure(model_name="7b", tokens=16384, samples_per_row=1, micro=2, steps=2, 
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="7b")
+    ap.add_argument("--model", default="7b", choices=["7b", "1.5b", "tiny"],
+                    help="7b: fp32 master + Adam moments + fp32 gradients alone are 16 B x 7.6e9 params = 122 GB, more than one 80 GB H100 holds")
     ap.add_argument("--tokens", type=int, default=16384)
     ap.add_argument("--samples-per-row", type=int, default=1)
     ap.add_argument("--micro", type=int, default=2, help="micro-batches per optimizer step")
