@@ -486,6 +486,22 @@ int prl_sample_logprob(const float* logits /*[B,V]*/, int32_t B, int32_t V, floa
 int prl_sample_logprob_rows(const float* logits /*[B,V]*/, int32_t B, int32_t V, const float* inv_temperature_rows,
                             const uint8_t* greedy_rows, uint64_t seed, uint32_t step, int32_t* out_ids,
                             float* out_logprobs, void* workspace, size_t workspace_bytes, prl_stream_t stream);
+/* Same with per-sequence top-k / top-p truncation (vLLM's rule under logprobs-mode processed_logprobs).  For a random
+ * row with z = logits * inv_temperature: top-k (active for 1 <= top_k_rows[b] < V) keeps { z >= k-th largest z }, ties
+ * included; top-p (active for top_p_rows[b] < 1) then keeps token i of that set S iff the mass of S strictly above z_i is
+ * < p * (mass of S).  id ~ softmax over the kept set (Gumbel-max with the noise of prl_sample_logprob_rows, so the id is
+ * the untruncated sampler's whenever that id is kept); logprob = z[id] - logsumexp(z over the kept set).  Greedy rows and
+ * rows without active truncation come out bit-identical to prl_sample_logprob_rows.  Optional per-row outputs (NULL to
+ * skip): out_kept = size of the kept set, out_threshold = its smallest z, out_log_norm = logsumexp over it (0, -inf and
+ * NaN for rows that are not truncated).  V <= 262 144; the caller validates top_k >= -1 and 0 < top_p <= 1.
+ * csrc/sample_topkp.cu: one 8-CTA cluster per row, radix selects merged through distributed shared memory. */
+size_t prl_sample_topkp_workspace_bytes(int32_t B, int32_t V);
+int prl_sample_logprob_topkp_rows(const float* logits /*[B,V]*/, int32_t B, int32_t V, const float* inv_temperature_rows,
+                                  const uint8_t* greedy_rows, const int32_t* top_k_rows, const float* top_p_rows,
+                                  uint64_t seed, uint32_t step, int32_t* out_ids, float* out_logprobs,
+                                  int32_t* out_kept /*[B] or NULL*/, float* out_threshold /*[B] or NULL*/,
+                                  float* out_log_norm /*[B] or NULL*/, void* workspace, size_t workspace_bytes,
+                                  prl_stream_t stream);
 /* Device-resident scheduler state of one sampler (all pointers device, one entry per slot).
  * prl_advance_state moves every active slot one token forward without a host round trip:
  * feeds the next prompt token while inside the prompt, else appends (sampled id, logprob) to the

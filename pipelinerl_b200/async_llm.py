@@ -2,10 +2,10 @@
 (reference: pipelinerl/async_llm.py:86-212 and :215-346)."""
 from __future__ import annotations
 
-from .engine import SamplingParams
+from .engine import SamplingParams, requested_truncation, truncation_params
 from .llm import LLMCall, LLMOutput, Prompt, TokenLogprob, TrainableLLM
 from .rollouts import TrainingText, apply_rollout_reward
-from .serving import resolve
+from .serving import resolve, sampling_features
 
 MASKED_TOKEN_ID = -100
 
@@ -34,12 +34,17 @@ def _chat_kwargs(llm: TrainableLLM, prompt: Prompt) -> dict:
     return kw
 
 
-def _reject_unsupported_sampling(params: dict) -> None:
+def _reject_unsupported_sampling(params: dict, features: frozenset = frozenset()) -> tuple[int, float]:
     """Sampling features the engine does not implement must fail loudly, exactly as http_shim.py answers 400 for them:
     a silently ignored top_p / top_k / stop would make the recorded logprobs those of a different distribution than the
-    one the request asked for.  (The reference trains with top_p = 1, top_k = -1, no stop strings: conf/base.yaml:46-51.)"""
-    if float(params.get("top_p", 1.0)) < 1.0 or int(params.get("top_k", -1)) > 0:
-        raise ValueError("top_p / top_k sampling is not implemented by this engine")
+    one the request asked for.  top_k / top_p are accepted when the target engine lists them in `features` (the unfused
+    single-GPU DecodeEngine does; the reference's eval handles send top_p 0.95 / top_k 50, conf/base.yaml:52-57); they
+    are validated as vLLM validates them.  Returns the request's (top_k, top_p)."""
+    greedy = float(params.get("temperature", 1.0)) <= 0
+    top_k, top_p = truncation_params(params, greedy=greedy)
+    missing = requested_truncation(top_k, top_p) - features
+    if missing:
+        raise ValueError(f"{' / '.join(sorted(missing))} sampling is not implemented by this engine")
     if params.get("stop") or params.get("stop_token_ids"):
         raise ValueError("stop strings / stop token ids are not implemented by this engine (eos only)")
     if int(params.get("n", 1)) != 1:
@@ -47,6 +52,7 @@ def _reject_unsupported_sampling(params: dict) -> None:
     for name in ("presence_penalty", "frequency_penalty", "repetition_penalty", "min_p"):
         if params.get(name) not in (None, 0, 0.0, 1, 1.0) or (name == "repetition_penalty" and params.get(name) not in (None, 1, 1.0)):
             raise ValueError(f"sampling parameter {name} is not implemented by this engine")
+    return top_k, top_p
 
 
 async def llm_async_generate(llm: TrainableLLM, prompt: Prompt, session=None,
@@ -58,11 +64,12 @@ async def llm_async_generate(llm: TrainableLLM, prompt: Prompt, session=None,
     prompt_ids = prompt.token_ids or _token_ids(tok.apply_chat_template(prompt.messages, add_generation_prompt=True,
                                                                         **_chat_kwargs(llm, prompt)))
     params = llm.parameters
-    _reject_unsupported_sampling(params)
+    top_k, top_p = _reject_unsupported_sampling(params, sampling_features(llm.base_url))
     max_tokens = int(max_tokens_override if max_tokens_override is not None else params.get("max_tokens", 16))
     temperature = float(params.get("temperature", 1.0))
     sp = SamplingParams(max_tokens=max_tokens, temperature=temperature if temperature > 0 else 1.0,
-                        greedy=temperature <= 0, ignore_eos=bool(params.get("ignore_eos", False)))
+                        greedy=temperature <= 0, ignore_eos=bool(params.get("ignore_eos", False)), top_k=top_k,
+                        top_p=top_p)
     req = await resolve(llm.base_url).generate(list(prompt_ids), sp)
     content = tok.decode(req.output_ids)
     call = llm.log_output(prompt, LLMOutput(content=content), count_tokens=False)

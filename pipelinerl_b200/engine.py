@@ -32,6 +32,31 @@ class SamplingParams:
     temperature: float = 1.0
     greedy: bool = False
     ignore_eos: bool = False
+    top_k: int = -1          # -1 / 0: off; 1 <= k < vocabulary: keep the k largest logits (and every tie of the k-th)
+    top_p: float = 1.0       # 1: off; else keep the smallest top set holding mass >= top_p (vLLM's rule)
+
+
+def truncation_params(params: dict, greedy: bool = False) -> tuple[int, float]:
+    """(top_k, top_p) of a request body / `llm.parameters`, validated as vLLM validates them (sampling_params.py:
+    top_p in (0, 1], top_k an int >= -1; a missing or None value is "off").  Greedy requests get (-1, 1.0): vLLM resets
+    truncation at temperature 0 after validating it.  Raises ValueError."""
+    top_k, top_p = params.get("top_k"), params.get("top_p")
+    top_k = -1 if top_k is None else top_k
+    top_p = 1.0 if top_p is None else top_p
+    if isinstance(top_k, bool) or not isinstance(top_k, int):
+        raise ValueError(f"top_k must be an integer, got {type(top_k).__name__}")
+    if top_k < -1:
+        raise ValueError(f"top_k must be -1 or 0 (disable), or at least 1, got {top_k}")
+    if isinstance(top_p, bool) or not isinstance(top_p, (int, float)) or not 0.0 < float(top_p) <= 1.0:
+        raise ValueError(f"top_p must be in (0, 1], got {top_p!r}")
+    if greedy:
+        return -1, 1.0
+    return int(top_k), float(top_p)
+
+
+def requested_truncation(top_k: int, top_p: float) -> set[str]:
+    """The truncation features a validated (top_k, top_p) pair asks for."""
+    return ({"top_k"} if top_k > 0 else set()) | ({"top_p"} if top_p < 1.0 else set())
 
 
 @dataclass
@@ -124,6 +149,11 @@ class DecodeEngine:
         self.inv_temp_rows = torch.ones(B, dtype=torch.float32, device=d)
         self.greedy_rows = torch.zeros(B, dtype=torch.uint8, device=d)
         self.ignore_eos_rows = torch.zeros(B, dtype=torch.uint8, device=d)
+        # top-k / top-p per slot; the truncated sampler runs only while some slot in _truncated_slots asks for it, so a
+        # batch without truncation launches exactly the untruncated sampler
+        self.top_k_rows = torch.full((B,), -1, dtype=torch.int32, device=d)
+        self.top_p_rows = torch.ones(B, dtype=torch.float32, device=d)
+        self._truncated_slots: set[int] = set()
         self._temperature, self._greedy, self._ignore_eos = 1.0, False, False
         self._graphs: dict[int, torch.cuda.CUDAGraph] = {}
         # ---- chunked prefill + prefix sharing (GRPO attempts share their prompt) ----
@@ -142,6 +172,12 @@ class DecodeEngine:
         self.profile_timing = False                    # benches: wall time spent inside run_prefill (costs two syncs per call)
         self._next_id = 0
         self._state = self._make_state()
+
+    @property
+    def sampling_features(self) -> frozenset:
+        """Truncation this engine samples with (`add_request` refuses the rest): the unfused sampler implements top-k and
+        top-p; the fused sampling head does not."""
+        return frozenset() if self.fused_head else frozenset({"top_k", "top_p"})
 
     # engine-wide sampling defaults: assigning one overwrites every slot (benches, tools, single-tenant tests)
     @property
@@ -286,10 +322,18 @@ class DecodeEngine:
                                             self.head_ws.data_ptr(), self.head_ws.numel(), st))
             _lib.check(lib.prl_advance_state(C.byref(self._state), st))
             return
-        _lib.check(lib.prl_sample_logprob_rows(self.logits.data_ptr(), self.B, self.cfg.head_rows,
-                                               self.inv_temp_rows.data_ptr(), self.greedy_rows.data_ptr(), self.seed,
-                                               self.step_count, self.sampled.data_ptr(), self.sampled_lp.data_ptr(),
-                                               self.sample_ws.data_ptr(), self.sample_ws.numel(), st))
+        if self._truncated_slots:
+            _lib.check(lib.prl_sample_logprob_topkp_rows(self.logits.data_ptr(), self.B, self.cfg.head_rows,
+                                                         self.inv_temp_rows.data_ptr(), self.greedy_rows.data_ptr(),
+                                                         self.top_k_rows.data_ptr(), self.top_p_rows.data_ptr(), self.seed,
+                                                         self.step_count, self.sampled.data_ptr(), self.sampled_lp.data_ptr(),
+                                                         None, None, None, self.sample_ws.data_ptr(), self.sample_ws.numel(),
+                                                         st))
+        else:
+            _lib.check(lib.prl_sample_logprob_rows(self.logits.data_ptr(), self.B, self.cfg.head_rows,
+                                                   self.inv_temp_rows.data_ptr(), self.greedy_rows.data_ptr(), self.seed,
+                                                   self.step_count, self.sampled.data_ptr(), self.sampled_lp.data_ptr(),
+                                                   self.sample_ws.data_ptr(), self.sample_ws.numel(), st))
         _lib.check(lib.prl_advance_state(C.byref(self._state), st))
 
     def step(self) -> None:
@@ -577,6 +621,11 @@ class DecodeEngine:
         if self.fused_head and (params.greedy != self._greedy or (not params.greedy and params.temperature != self._temperature)):
             raise ValueError("the fused sampling head takes engine-wide sampling parameters: build the engine with "
                              "fused_head=False to mix requests with different temperature / greedy settings")
+        top_k, top_p = truncation_params({"top_k": params.top_k, "top_p": params.top_p}, greedy=params.greedy)
+        missing = requested_truncation(top_k, top_p) - self.sampling_features
+        if missing:
+            raise ValueError(f"{' / '.join(sorted(missing))} sampling is not implemented by this engine "
+                             f"({type(self).__name__}, fused_head={self.fused_head})")
         if not self.can_admit(n, params.max_tokens):
             raise RuntimeError("engine full")
         req = Request(self._next_id, list(prompt_ids), params, model_version=model_version)
@@ -629,6 +678,10 @@ class DecodeEngine:
         self.max_new_t[slot] = params.max_tokens
         self.inv_temp_rows[slot] = 1.0 if params.greedy else 1.0 / float(params.temperature)
         self.greedy_rows[slot] = int(bool(params.greedy))
+        self.top_k_rows[slot] = top_k
+        self.top_p_rows[slot] = top_p
+        if requested_truncation(top_k, top_p):
+            self._truncated_slots.add(slot)
         self.ignore_eos_rows[slot] = int(bool(params.ignore_eos) or self._ignore_eos)
         self.tokens[slot] = prompt_ids[start]
         self.positions[slot] = start
@@ -655,6 +708,10 @@ class DecodeEngine:
             req.finish_reason = "stop" if code == 1 else "length"
             self.block_table[slot].zero_()
             self.finished[slot] = 0
+            if slot in self._truncated_slots:
+                self._truncated_slots.discard(slot)
+                self.top_k_rows[slot] = -1
+                self.top_p_rows[slot] = 1.0
             self._release_pages(req.pages)
             self.free_slots.append(slot)
             del self.slot_req[slot]

@@ -17,8 +17,11 @@ at this shim instead of a vLLM server (SURVEY §8b "wire format"):
   POST /receive_weight_update the reference's trigger for its NCCL broadcast (vllm1.py:244-249).  Here weights arrive by
                               the learner's P2P push; the endpoint only reports the version the sampler is serving.
 
-Sampling features the engine does not implement (top_p < 1, top_k > 0, n > 1, streaming) are rejected with 400 rather
-than silently ignored.  Host code only: the engine behind it is the CUDA DecodeEngine (no CPU fallback).
+top_k / top_p are served when the engine lists them in `engine.sampling_features` (the unfused single-GPU DecodeEngine:
+vLLM's truncation rule, with the logprob of the truncated distribution) and are validated as vLLM validates them.
+Sampling features the engine does not implement (truncation on the fused-head or TP engines, n > 1, streaming) are
+rejected with 400 rather than silently ignored.  Host code only: the engine behind it is the CUDA DecodeEngine (no CPU
+fallback).
 """
 from __future__ import annotations
 
@@ -30,7 +33,7 @@ from typing import Any
 
 from aiohttp import web
 
-from .engine import SamplingParams
+from .engine import SamplingParams, requested_truncation, truncation_params
 
 
 def _token_ids(encoded) -> list[int]:
@@ -103,15 +106,20 @@ class HttpShim:
         return web.json_response({"error": {"message": msg, "type": "invalid_request_error"}}, status=400)
 
     def _sampling(self, body: dict) -> SamplingParams | web.Response:
-        if float(body.get("top_p", 1.0)) < 1.0 or int(body.get("top_k", -1)) > 0:
-            return self._bad("top_p / top_k sampling is not implemented by this engine (the reference trains with "
-                             "top_p=1, top_k=-1, conf/base.yaml:46-51)")
+        temperature = float(body.get("temperature", 1.0))
+        try:
+            top_k, top_p = truncation_params(body, greedy=temperature <= 0)
+        except ValueError as e:
+            return self._bad(str(e))
+        engine = getattr(self.server, "engine", None)
+        missing = requested_truncation(top_k, top_p) - frozenset(getattr(engine, "sampling_features", frozenset()))
+        if missing:
+            return self._bad(f"{' / '.join(sorted(missing))} sampling is not implemented by this engine")
         if int(body.get("n", 1)) != 1 or body.get("stream"):
             return self._bad("n > 1 and streaming are not implemented")
-        temperature = float(body.get("temperature", 1.0))
         max_tokens = int(body.get("max_tokens") or body.get("max_completion_tokens") or self.default_max_tokens)
         return SamplingParams(max_tokens=max_tokens, temperature=temperature if temperature > 0 else 1.0,
-                              greedy=temperature <= 0)
+                              greedy=temperature <= 0, top_k=top_k, top_p=top_p)
 
     async def chat_completions(self, request: web.Request) -> web.Response:
         body = await request.json()

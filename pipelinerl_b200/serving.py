@@ -27,6 +27,16 @@ def resolve(base_url: str) -> "EngineServer":
     return _REGISTRY[name]
 
 
+def sampling_features(base_url: str) -> frozenset:
+    """Truncation features ("top_k", "top_p") the engine registered at `base_url` implements; empty when nothing is
+    registered there or its engine does not list any, so clients refuse such requests instead of ignoring them."""
+    try:
+        server = resolve(base_url)
+    except (ValueError, KeyError):
+        return frozenset()
+    return frozenset(getattr(getattr(server, "engine", None), "sampling_features", frozenset()))
+
+
 @dataclass
 class _Pending:
     prompt_ids: list[int]

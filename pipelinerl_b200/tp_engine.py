@@ -27,6 +27,10 @@ from .weights import ipc_alloc, ipc_export, ipc_open
 
 
 class TPDecodeEngine(DecodeEngine):
+    # the vocab-parallel head exchanges 16 sampler partials per row, not logits: no rank sees the whole row that a
+    # top-k / top-p threshold is taken over, so add_request refuses truncation here
+    sampling_features = frozenset()
+
     def __init__(self, full_cfg: ModelConfig, arena: ParamArena, tp_rank: int, tp_size: int, group=None, **kw):
         import torch.distributed as dist
         if tp_size < 2 or tp_size > 8:
