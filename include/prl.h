@@ -320,6 +320,21 @@ int prl_colsum_bf16(const void* x, int64_t ld, int64_t T, int64_t cols, float* o
  * sign = +1 forward, -1 backward (the transpose of a rotation) */
 int prl_rope_inplace(void* x, int64_t ld, int64_t T, int32_t n_heads, int32_t head_dim, const int32_t* pos,
                      const float* inv_freq /*[head_dim/2]*/, float sign, prl_stream_t stream);
+/* Qwen3 learner: heads [0, n_q) (q) and [n_q, n_q + n_kv) (k) of every row of qkv [T, ld] in place: per-head RMSNorm
+ * with gain q_gamma / k_gamma ([128] bf16), then RoPE, in fp32, rounded to bf16 once (replaces prl_rope_inplace for
+ * these models).  With qk_pre [T, (n_q + n_kv) * 128] bf16 and rstd [T, n_q + n_kv] fp32 (both or neither), the
+ * pre-norm q | k columns and the per-head 1 / rms are kept for the backward. */
+int prl_qk_norm_rope_fwd(void* qkv, int64_t ld, int64_t T, int32_t n_q, int32_t n_kv, int32_t head_dim,
+                         const void* q_gamma, const void* k_gamma, float eps, const int32_t* pos,
+                         const float* inv_freq /*[head_dim/2]*/, void* qk_pre /*or NULL*/, float* rstd /*or NULL*/,
+                         prl_stream_t stream);
+/* Its backward on dqkv [T, ld] in place (q | k columns: inverse rotation, then the RMSNorm backward);
+ * dq_gamma / dk_gamma ([128] fp32) += the gain gradients, summed in a fixed order (per-block partials, then one pass).
+ * workspace >= prl_rowops_workspace_bytes(256). */
+int prl_qk_norm_rope_bwd(void* dqkv, int64_t ld, int64_t T, int32_t n_q, int32_t n_kv, int32_t head_dim,
+                         const void* q_gamma, const void* k_gamma, const int32_t* pos, const float* inv_freq,
+                         const void* qk_pre, const float* rstd, float* dq_gamma, float* dk_gamma, void* workspace,
+                         size_t workspace_bytes, prl_stream_t stream);
 /* gate_up [T, 2I] = [gate | up] -> act [T, I] = silu(gate) * up, and its backward */
 int prl_silu_mul_fwd(const void* gate_up, int64_t T, int64_t I, void* act, prl_stream_t stream);
 int prl_silu_mul_bwd(const void* gate_up, const void* dact, int64_t T, int64_t I, void* dgate_up, prl_stream_t stream);
@@ -401,6 +416,15 @@ int prl_qkv_rope_cache(const float* partials, int32_t n_split, int32_t B, const 
                        const float* inv_freq /*[head_dim/2]*/, void* q_out_bf16 /*[B,n_q,128]*/,
                        void* kv_cache_bf16, int64_t n_pages, int32_t layer, int32_t page_size,
                        const void* l2_prefetch, size_t l2_prefetch_bytes, prl_stream_t stream);
+/* Qwen3: the same step with a per-head RMSNorm of every q and k head before RoPE.  In fp32, per head: split-K sum,
+ * bias, x * rsqrt(sum(x^2)/128 + eps) * gamma (q_gamma_bf16 for q heads, k_gamma_bf16 for k heads, [128] each),
+ * rotation, one rounding to bf16; v heads untouched.  Both gains NULL = prl_qkv_rope_cache, bit for bit. */
+int prl_qkv_norm_rope_cache(const float* partials, int32_t n_split, int32_t B, const void* bias_bf16 /*or NULL*/,
+                            const void* q_gamma_bf16, const void* k_gamma_bf16, float eps, int32_t n_q, int32_t n_kv,
+                            int32_t head_dim, const int32_t* positions, const int32_t* block_table, int32_t max_blocks,
+                            const int32_t* row_slot, const float* inv_freq, void* q_out_bf16, void* kv_cache_bf16,
+                            int64_t n_pages, int32_t layer, int32_t page_size, const void* l2_prefetch,
+                            size_t l2_prefetch_bytes, prl_stream_t stream);
 int prl_silu_mul(const float* partials, int32_t n_split, int32_t B, int32_t I, void* act_bf16 /*[B,I]*/,
                  const void* l2_prefetch, size_t l2_prefetch_bytes, prl_stream_t stream);
 int prl_paged_attn_splits(int32_t B, int32_t n_kv, int32_t max_seq_len);

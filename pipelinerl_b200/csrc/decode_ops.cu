@@ -118,11 +118,34 @@ __global__ void __launch_bounds__(1024) residual_rmsnorm_kernel(const float* __r
   }
 }
 
-// ---- split-K reduce + bias + RoPE + KV-page write ---------------------------------------
+// ---- split-K reduce + bias (+ per-head q/k RMSNorm) + RoPE + KV-page write ------------------------
 // part [n_split, B, (n_q + 2 n_kv) * 128]; one block per (token, head), 64 threads = 64 rotation pairs.
 // q -> q_out [B, n_q, 128] bf16 ; k, v -> cache rows ((layer*2 + kv) * n_pages + page) * n_kv * PAGE + kvh*PAGE + slot
+// kNorm (Qwen3): every q and k head is RMS-normalised over its 128 values and scaled by the layer's gain (q_gamma for
+// q heads, k_gamma for k heads) before the rotation, all in fp32; v heads are untouched.  Values are rounded to bf16
+// once, after RoPE.  The kNorm = false instantiation is the Qwen2 step, unchanged.
+
+// Sum of squares of one head's 128 values, held as pairs (x1, x2) by 64 consecutive threads (two whole warps): one
+// butterfly per warp, then the two warp sums in order.  Both kernels below reduce in exactly this order, so they stay
+// bit-identical.  Block-wide: every thread of the block must call it.
+__device__ __forceinline__ float head_sumsq(float x1, float x2, float* s_ss) {
+  float v = warp_sum(__fadd_rn(__fmul_rn(x1, x1), __fmul_rn(x2, x2)));
+  const int warp = threadIdx.x >> 5;
+  __syncthreads();  // s_ss may still be read from the previous head
+  if ((threadIdx.x & 31) == 0) s_ss[warp] = v;
+  __syncthreads();
+  const int w0 = warp & ~1;
+  return __fadd_rn(s_ss[w0], s_ss[w0 + 1]);
+}
+
+__device__ __forceinline__ float head_rstd(float ss, float eps) { return rsqrtf(__fmaf_rn(ss, 1.f / 128.f, eps)); }
+
+template <bool kNorm>
 __global__ void __launch_bounds__(64) qkv_rope_cache_kernel(const float* __restrict__ part, int n_split, int B,
-                                                           const __nv_bfloat16* __restrict__ bias, int n_q, int n_kv,
+                                                           const __nv_bfloat16* __restrict__ bias,
+                                                           const __nv_bfloat16* __restrict__ q_gamma,
+                                                           const __nv_bfloat16* __restrict__ k_gamma, float eps,
+                                                           int n_q, int n_kv,
                                                            const int32_t* __restrict__ positions,
                                                            const int32_t* __restrict__ block_table, int max_blocks,
                                                            const int32_t* __restrict__ row_slot,
@@ -151,9 +174,16 @@ __global__ void __launch_bounds__(64) qkv_rope_cache_kernel(const float* __restr
     x2 += __bfloat162float(bias[col + 64]);
   }
   const int pos = positions[b];
-  const bool is_v = head >= n_q + n_kv;
+  const bool is_v = head >= n_q + n_kv;  // uniform over the block
   float o1 = x1, o2 = x2;
   if (!is_v) {
+    if constexpr (kNorm) {
+      __shared__ float s_ss[2];
+      const float r = head_rstd(head_sumsq(x1, x2, s_ss), eps);
+      const __nv_bfloat16* g = head < n_q ? q_gamma : k_gamma;
+      x1 = x1 * r * __bfloat162float(g[i]);
+      x2 = x2 * r * __bfloat162float(g[i + 64]);
+    }
     // NeoX-style rotation of the pair (i, i + 64); inv_freq[i] = 1 / theta^(2i/128) is tabulated by the host
     // with the exact fp32 expression HF's rotary embedding uses, the angle is an fp32 product as there
     const float inv_freq = inv_freq_tab[i];
@@ -182,8 +212,13 @@ __global__ void __launch_bounds__(64) qkv_rope_cache_kernel(const float* __restr
 // Same arithmetic, laid out for MANY rows (prefill chunks): one block walks whole token rows, the row's 64
 // (cos, sin) pairs are computed once (the per-head kernel above recomputes them for each of the n_q + 2 n_kv heads)
 // and every thread handles (head, pair) items with coalesced 4-byte loads.  Bitwise identical results.
+// blockDim must be a multiple of 64, so that each head's 64 pairs are two whole warps of one pass (head_sumsq).
+template <bool kNorm>
 __global__ void __launch_bounds__(256) qkv_rope_cache_rows_kernel(const float* __restrict__ part, int n_split, int B,
-                                                                const __nv_bfloat16* __restrict__ bias, int n_q, int n_kv,
+                                                                const __nv_bfloat16* __restrict__ bias,
+                                                                const __nv_bfloat16* __restrict__ q_gamma,
+                                                                const __nv_bfloat16* __restrict__ k_gamma, float eps,
+                                                                int n_q, int n_kv,
                                                                 const int32_t* __restrict__ positions,
                                                                 const int32_t* __restrict__ block_table, int max_blocks,
                                                                 const int32_t* __restrict__ row_slot,
@@ -195,6 +230,7 @@ __global__ void __launch_bounds__(256) qkv_rope_cache_rows_kernel(const float* _
   pdl_wait();
   constexpr int D = 128;
   __shared__ float s_cs[64], s_sn[64];
+  __shared__ float s_ss[kNorm ? 256 / 32 : 1];
   const int n_heads = n_q + 2 * n_kv;
   const int64_t ncol = (int64_t)n_heads * D;
   for (int b = blockIdx.x; b < B; b += gridDim.x) {
@@ -210,20 +246,34 @@ __global__ void __launch_bounds__(256) qkv_rope_cache_rows_kernel(const float* _
     const int slot_row = row_slot ? row_slot[b] : b;
     const int page = block_table[(int64_t)slot_row * max_blocks + pos / page_size];
     const int slot = pos % page_size;
-    for (int w = threadIdx.x; w < n_heads * 64; w += blockDim.x) {
+    // every thread runs every pass (the norm's reduction is block-wide); threads past the last head only idle
+    for (int w0 = 0; w0 < n_heads * 64; w0 += blockDim.x) {
+      const int w = w0 + threadIdx.x;
+      const bool live = w < n_heads * 64;
       const int head = w >> 6, i = w & 63;
       const int col = head * D + i;
       float x1 = 0.f, x2 = 0.f;
-      for (int s = 0; s < n_split; ++s) {
-        const float* p = part + ((int64_t)s * B + b) * ncol;
-        x1 += p[col];
-        x2 += p[col + 64];
-      }
-      if (bias) {
-        x1 += __bfloat162float(bias[col]);
-        x2 += __bfloat162float(bias[col + 64]);
+      if (live) {
+        for (int s = 0; s < n_split; ++s) {
+          const float* p = part + ((int64_t)s * B + b) * ncol;
+          x1 += p[col];
+          x2 += p[col + 64];
+        }
+        if (bias) {
+          x1 += __bfloat162float(bias[col]);
+          x2 += __bfloat162float(bias[col + 64]);
+        }
       }
       const bool is_v = head >= n_q + n_kv;
+      if constexpr (kNorm) {
+        const float r = head_rstd(head_sumsq(x1, x2, s_ss), eps);
+        if (live && !is_v) {
+          const __nv_bfloat16* g = head < n_q ? q_gamma : k_gamma;
+          x1 = x1 * r * __bfloat162float(g[i]);
+          x2 = x2 * r * __bfloat162float(g[i + 64]);
+        }
+      }
+      if (!live) continue;
       float o1 = x1, o2 = x2;
       if (!is_v) {
         const float cs = s_cs[i], sn = s_sn[i];
@@ -473,31 +523,46 @@ extern "C" int prl_residual_rmsnorm(const float* partials, int32_t n_split, int3
   return PRL_OK;
 }
 
+extern "C" int prl_qkv_norm_rope_cache(const float* partials, int32_t n_split, int32_t B, const void* bias,
+                                       const void* q_gamma, const void* k_gamma, float eps, int32_t n_q, int32_t n_kv,
+                                       int32_t head_dim, const int32_t* positions, const int32_t* block_table,
+                                       int32_t max_blocks, const int32_t* row_slot, const float* inv_freq, void* q_out,
+                                       void* kv_cache, int64_t n_pages, int32_t layer, int32_t page_size,
+                                       const void* l2_prefetch, size_t l2_prefetch_bytes, prl_stream_t st) {
+  PRL_CHECK_ARG(partials && positions && block_table && q_out && kv_cache && inv_freq, "prl_qkv_rope_cache: NULL argument");
+  PRL_CHECK_ARG(head_dim == 128, "prl_qkv_rope_cache: head_dim must be 128 (got %d)", head_dim);
+  PRL_CHECK_ARG(B >= 1 && n_q >= 1 && n_kv >= 1 && page_size >= 1 && max_blocks >= 1, "prl_qkv_rope_cache: bad shape");
+  PRL_CHECK_ARG((q_gamma == nullptr) == (k_gamma == nullptr),
+                "prl_qkv_norm_rope_cache: q_gamma and k_gamma must both be given (q/k norm) or both be NULL");
+  const bool norm = q_gamma != nullptr;
+  const __nv_bfloat16 *qg = (const __nv_bfloat16*)q_gamma, *kg = (const __nv_bfloat16*)k_gamma;
+  if (B > 128) {  // prefill chunk: row-walking variant (same results, ~4x less time at 1024 rows)
+    const unsigned blocks = (unsigned)(B < 132 * 8 ? B : 132 * 8);
+    PRL_CUDA(launch_pdl(norm ? qkv_rope_cache_rows_kernel<true> : qkv_rope_cache_rows_kernel<false>, dim3(blocks),
+                        dim3(256), 0, (cudaStream_t)st, partials, (int)n_split, (int)B, (const __nv_bfloat16*)bias, qg, kg,
+                        eps, (int)n_q, (int)n_kv, positions, block_table, (int)max_blocks, row_slot, inv_freq,
+                        (__nv_bfloat16*)q_out, (__nv_bfloat16*)kv_cache, n_pages, (int)layer, (int)page_size));
+    PRL_LAUNCH_CHECK();
+    return PRL_OK;
+  }
+  dim3 grid((unsigned)B, (unsigned)(n_q + 2 * n_kv));
+  PRL_CUDA(launch_pdl(norm ? qkv_rope_cache_kernel<true> : qkv_rope_cache_kernel<false>, grid, dim3(64), 0,
+                      (cudaStream_t)st, partials, (int)n_split, (int)B, (const __nv_bfloat16*)bias, qg, kg, eps, (int)n_q,
+                      (int)n_kv, positions, block_table, (int)max_blocks, row_slot, inv_freq, (__nv_bfloat16*)q_out,
+                      (__nv_bfloat16*)kv_cache, n_pages, (int)layer, (int)page_size, l2_prefetch, l2_prefetch_bytes));
+  PRL_LAUNCH_CHECK();
+  return PRL_OK;
+}
+
 extern "C" int prl_qkv_rope_cache(const float* partials, int32_t n_split, int32_t B, const void* bias, int32_t n_q,
                                   int32_t n_kv, int32_t head_dim, const int32_t* positions,
                                   const int32_t* block_table, int32_t max_blocks, const int32_t* row_slot,
                                   const float* inv_freq, void* q_out,
                                   void* kv_cache, int64_t n_pages, int32_t layer, int32_t page_size,
                                   const void* l2_prefetch, size_t l2_prefetch_bytes, prl_stream_t st) {
-  PRL_CHECK_ARG(partials && positions && block_table && q_out && kv_cache && inv_freq, "prl_qkv_rope_cache: NULL argument");
-  PRL_CHECK_ARG(head_dim == 128, "prl_qkv_rope_cache: head_dim must be 128 (got %d)", head_dim);
-  PRL_CHECK_ARG(B >= 1 && n_q >= 1 && n_kv >= 1 && page_size >= 1 && max_blocks >= 1, "prl_qkv_rope_cache: bad shape");
-  if (B > 128) {  // prefill chunk: row-walking variant (same results, ~4x less time at 1024 rows)
-    const unsigned blocks = (unsigned)(B < 132 * 8 ? B : 132 * 8);
-    PRL_CUDA(launch_pdl(qkv_rope_cache_rows_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)st, partials, (int)n_split,
-                        (int)B, (const __nv_bfloat16*)bias, (int)n_q, (int)n_kv, positions, block_table, (int)max_blocks,
-                        row_slot, inv_freq, (__nv_bfloat16*)q_out, (__nv_bfloat16*)kv_cache, n_pages, (int)layer,
-                        (int)page_size));
-    PRL_LAUNCH_CHECK();
-    return PRL_OK;
-  }
-  dim3 grid((unsigned)B, (unsigned)(n_q + 2 * n_kv));
-  PRL_CUDA(launch_pdl(qkv_rope_cache_kernel, grid, dim3(64), 0, (cudaStream_t)st, partials, (int)n_split, (int)B,
-                      (const __nv_bfloat16*)bias, (int)n_q, (int)n_kv, positions, block_table, (int)max_blocks, row_slot,
-                      inv_freq, (__nv_bfloat16*)q_out, (__nv_bfloat16*)kv_cache, n_pages, (int)layer, (int)page_size,
-                      l2_prefetch, l2_prefetch_bytes));
-  PRL_LAUNCH_CHECK();
-  return PRL_OK;
+  return prl_qkv_norm_rope_cache(partials, n_split, B, bias, nullptr, nullptr, 0.f, n_q, n_kv, head_dim, positions,
+                                 block_table, max_blocks, row_slot, inv_freq, q_out, kv_cache, n_pages, layer, page_size,
+                                 l2_prefetch, l2_prefetch_bytes, st);
 }
 
 extern "C" int prl_silu_mul(const float* partials, int32_t n_split, int32_t B, int32_t I, void* act_bf16,

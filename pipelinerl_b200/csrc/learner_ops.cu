@@ -222,6 +222,158 @@ __global__ void rope_kernel(__nv_bfloat16* __restrict__ x, int64_t ld, int64_t T
   }
 }
 
+// ---- Qwen3: per-head RMSNorm of q and k, then RoPE (forward), and the backward of the pair ---------------------------
+// qkv [T, ld] bf16 in place; heads [0, n_q) are q, [n_q, n_q + n_kv) are k (v heads are not touched).  One block per
+// row (grid-stride), one warp per head: lane l owns the rotation pairs (2l, 2l + 64) and (2l + 1, 2l + 65).  Per head,
+// in fp32: y = x * rstd * gamma with rstd = rsqrt(mean(x^2) + eps), then the rotation, rounded to bf16 once.
+constexpr int kQkThreads = 256;
+
+__device__ __forceinline__ void load_pair4(const __nv_bfloat16* p, int lane, float (&v)[4]) {
+  const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p + 2 * lane));
+  const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p + 64 + 2 * lane));
+  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
+}
+__device__ __forceinline__ void store_pair4(__nv_bfloat16* p, int lane, const float (&v)[4]) {
+  *reinterpret_cast<__nv_bfloat162*>(p + 2 * lane) = __floats2bfloat162_rn(v[0], v[1]);
+  *reinterpret_cast<__nv_bfloat162*>(p + 64 + 2 * lane) = __floats2bfloat162_rn(v[2], v[3]);
+}
+
+// x_pre [T, (n_q + n_kv) * 128] (nullable): the pre-norm q | k columns, kept for the backward; rstd [T, n_q + n_kv]
+__global__ void __launch_bounds__(kQkThreads) qk_norm_rope_fwd_kernel(__nv_bfloat16* __restrict__ x, int64_t ld,
+                                                                      int64_t T, int n_q, int n_kv,
+                                                                      const __nv_bfloat16* __restrict__ q_gamma,
+                                                                      const __nv_bfloat16* __restrict__ k_gamma, float eps,
+                                                                      const int32_t* __restrict__ pos,
+                                                                      const float* __restrict__ inv_freq,
+                                                                      __nv_bfloat16* __restrict__ x_pre,
+                                                                      float* __restrict__ rstd) {
+  __shared__ float s_cs[64], s_sn[64];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+  const int nh = n_q + n_kv;
+  float gq[4], gk[4];
+  load_pair4(q_gamma, lane, gq);
+  load_pair4(k_gamma, lane, gk);
+  for (int64_t row = blockIdx.x; row < T; row += gridDim.x) {
+    __syncthreads();
+    if (threadIdx.x < 64) {
+      float sn, cs;
+      sincosf((float)pos[row] * inv_freq[threadIdx.x], &sn, &cs);
+      s_cs[threadIdx.x] = cs;
+      s_sn[threadIdx.x] = sn;
+    }
+    __syncthreads();
+    const float c0 = s_cs[2 * lane], c1 = s_cs[2 * lane + 1], s0 = s_sn[2 * lane], s1 = s_sn[2 * lane + 1];
+    for (int head = warp; head < nh; head += n_warps) {
+      __nv_bfloat16* p = x + row * ld + (int64_t)head * 128;
+      float v[4];
+      load_pair4(p, lane, v);
+      if (x_pre) {
+        __nv_bfloat16* q = x_pre + (row * nh + head) * 128;
+        *reinterpret_cast<__nv_bfloat162*>(q + 2 * lane) = *reinterpret_cast<const __nv_bfloat162*>(p + 2 * lane);
+        *reinterpret_cast<__nv_bfloat162*>(q + 64 + 2 * lane) = *reinterpret_cast<const __nv_bfloat162*>(p + 64 + 2 * lane);
+      }
+      const float ss = warp_sum(v[0] * v[0] + v[1] * v[1] + v[2] * v[2] + v[3] * v[3]);
+      const float r = rsqrtf(ss * (1.f / 128.f) + eps);
+      if (rstd && lane == 0) rstd[row * nh + head] = r;
+      const bool is_q = head < n_q;
+      float y[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) y[e] = v[e] * r * (is_q ? gq[e] : gk[e]);
+      float o[4];
+      o[0] = y[0] * c0 - y[2] * s0;
+      o[2] = y[2] * c0 + y[0] * s0;
+      o[1] = y[1] * c1 - y[3] * s1;
+      o[3] = y[3] * c1 + y[1] * s1;
+      store_pair4(p, lane, o);
+    }
+  }
+}
+
+// dx (the gradient of the roped q | k columns of dqkv, in place) -> inverse rotation -> RMSNorm backward:
+//   dx = rstd * (g * dy - xhat * mean(xhat * g * dy)),  dgamma += sum over rows and heads of dy * xhat (q and k apart)
+// partial[block][256] = this block's gain sums (q: [0, 128), k: [128, 256)), summed over its warps in a fixed order.
+__global__ void __launch_bounds__(kQkThreads) qk_norm_rope_bwd_kernel(__nv_bfloat16* __restrict__ dx, int64_t ld,
+                                                                      int64_t T, int n_q, int n_kv,
+                                                                      const __nv_bfloat16* __restrict__ q_gamma,
+                                                                      const __nv_bfloat16* __restrict__ k_gamma,
+                                                                      const int32_t* __restrict__ pos,
+                                                                      const float* __restrict__ inv_freq,
+                                                                      const __nv_bfloat16* __restrict__ x_pre,
+                                                                      const float* __restrict__ rstd,
+                                                                      float* __restrict__ partial) {
+  __shared__ float s_cs[64], s_sn[64];
+  __shared__ float s_acc[kQkThreads / 32][256];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+  const int nh = n_q + n_kv;
+  float gq[4], gk[4], aq[4] = {0.f, 0.f, 0.f, 0.f}, ak[4] = {0.f, 0.f, 0.f, 0.f};
+  load_pair4(q_gamma, lane, gq);
+  load_pair4(k_gamma, lane, gk);
+  for (int64_t row = blockIdx.x; row < T; row += gridDim.x) {
+    __syncthreads();
+    if (threadIdx.x < 64) {
+      float sn, cs;
+      sincosf((float)pos[row] * inv_freq[threadIdx.x], &sn, &cs);
+      s_cs[threadIdx.x] = cs;
+      s_sn[threadIdx.x] = sn;
+    }
+    __syncthreads();
+    const float c0 = s_cs[2 * lane], c1 = s_cs[2 * lane + 1], s0 = s_sn[2 * lane], s1 = s_sn[2 * lane + 1];
+    for (int head = warp; head < nh; head += n_warps) {
+      __nv_bfloat16* p = dx + row * ld + (int64_t)head * 128;
+      float d[4], xv[4];
+      load_pair4(p, lane, d);
+      load_pair4(x_pre + (row * nh + head) * 128, lane, xv);
+      float dy[4];  // the transpose of the rotation
+      dy[0] = d[0] * c0 + d[2] * s0;
+      dy[2] = d[2] * c0 - d[0] * s0;
+      dy[1] = d[1] * c1 + d[3] * s1;
+      dy[3] = d[3] * c1 - d[1] * s1;
+      const float r = rstd[row * nh + head];
+      const bool is_q = head < n_q;
+      float xh[4], gd[4], dot = 0.f;
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        xh[e] = xv[e] * r;
+        gd[e] = (is_q ? gq[e] : gk[e]) * dy[e];
+        dot += xh[e] * gd[e];
+      }
+      const float m = warp_sum(dot) * (1.f / 128.f);
+      float o[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[e] = r * (gd[e] - xh[e] * m);
+      store_pair4(p, lane, o);
+      if (is_q) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) aq[e] += dy[e] * xh[e];
+      } else {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) ak[e] += dy[e] * xh[e];
+      }
+    }
+  }
+  const int idx[4] = {2 * lane, 2 * lane + 1, 64 + 2 * lane, 65 + 2 * lane};
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    s_acc[warp][idx[e]] = aq[e];
+    s_acc[warp][128 + idx[e]] = ak[e];
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < 256; c += blockDim.x) {
+    float t = 0.f;
+    for (int w = 0; w < n_warps; ++w) t += s_acc[w][c];
+    partial[(int64_t)blockIdx.x * 256 + c] = t;
+  }
+}
+
+// dq_gamma[c] += sum_b partial[b][c], dk_gamma[c] += sum_b partial[b][128 + c], b ascending
+__global__ void __launch_bounds__(256) qk_gain_reduce_kernel(const float* __restrict__ partial, int n_blocks,
+                                                             float* __restrict__ dq_gamma, float* __restrict__ dk_gamma) {
+  const int c = threadIdx.x;
+  float s = 0.f;
+  for (int b = 0; b < n_blocks; ++b) s += partial[(int64_t)b * 256 + c];
+  if (c < 128) dq_gamma[c] += s; else dk_gamma[c - 128] += s;
+}
+
 __global__ void __launch_bounds__(256) silu_mul_fwd_kernel(const __nv_bfloat16* __restrict__ gu, int64_t T, int I,
                                                            __nv_bfloat16* __restrict__ act) {
   const int64_t nvec = T * (I >> 3);
@@ -354,6 +506,44 @@ extern "C" int prl_rope_inplace(void* x, int64_t ld, int64_t T, int32_t n_heads,
   threads = threads > 256 ? 256 : ((threads + 31) / 32 * 32);
   rope_kernel<<<(unsigned)(T < 8 * kPartialBlocks ? T : 8 * kPartialBlocks), threads, (size_t)head_dim * sizeof(float),
                 (cudaStream_t)stream>>>((__nv_bfloat16*)x, ld, T, n_heads, head_dim, pos, inv_freq, sign);
+  PRL_LAUNCH_CHECK();
+  return PRL_OK;
+}
+
+extern "C" int prl_qk_norm_rope_fwd(void* qkv, int64_t ld, int64_t T, int32_t n_q, int32_t n_kv, int32_t head_dim,
+                                    const void* q_gamma, const void* k_gamma, float eps, const int32_t* pos,
+                                    const float* inv_freq, void* qk_pre, float* rstd, prl_stream_t stream) {
+  PRL_CHECK_ARG(qkv && q_gamma && k_gamma && pos && inv_freq && T >= 1 && n_q >= 1 && n_kv >= 1,
+                "prl_qk_norm_rope_fwd: bad argument");
+  PRL_CHECK_ARG(head_dim == 128, "prl_qk_norm_rope_fwd: head_dim must be 128 (got %d)", head_dim);
+  PRL_CHECK_ARG(ld % 8 == 0 && ld >= (int64_t)(n_q + n_kv) * 128, "prl_qk_norm_rope_fwd: ld must be a multiple of 8 "
+                "covering the q | k heads");
+  PRL_CHECK_ARG((qk_pre == nullptr) == (rstd == nullptr), "prl_qk_norm_rope_fwd: qk_pre and rstd go together");
+  qk_norm_rope_fwd_kernel<<<(unsigned)(T < 4 * kPartialBlocks ? T : 4 * kPartialBlocks), kQkThreads, 0,
+                            (cudaStream_t)stream>>>((__nv_bfloat16*)qkv, ld, T, (int)n_q, (int)n_kv,
+                                                    (const __nv_bfloat16*)q_gamma, (const __nv_bfloat16*)k_gamma, eps, pos,
+                                                    inv_freq, (__nv_bfloat16*)qk_pre, rstd);
+  PRL_LAUNCH_CHECK();
+  return PRL_OK;
+}
+
+extern "C" int prl_qk_norm_rope_bwd(void* dqkv, int64_t ld, int64_t T, int32_t n_q, int32_t n_kv, int32_t head_dim,
+                                    const void* q_gamma, const void* k_gamma, const int32_t* pos, const float* inv_freq,
+                                    const void* qk_pre, const float* rstd, float* dq_gamma, float* dk_gamma,
+                                    void* workspace, size_t workspace_bytes, prl_stream_t stream) {
+  PRL_CHECK_ARG(dqkv && q_gamma && k_gamma && pos && inv_freq && qk_pre && rstd && dq_gamma && dk_gamma && workspace &&
+                    T >= 1 && n_q >= 1 && n_kv >= 1,
+                "prl_qk_norm_rope_bwd: bad argument");
+  PRL_CHECK_ARG(head_dim == 128, "prl_qk_norm_rope_bwd: head_dim must be 128 (got %d)", head_dim);
+  PRL_CHECK_ARG(ld % 8 == 0 && ld >= (int64_t)(n_q + n_kv) * 128, "prl_qk_norm_rope_bwd: ld must be a multiple of 8 "
+                "covering the q | k heads");
+  PRL_CHECK_ARG(workspace_bytes >= prl_rowops_workspace_bytes(256), "prl_qk_norm_rope_bwd: workspace too small");
+  const int g = row_grid(T);
+  qk_norm_rope_bwd_kernel<<<g, kQkThreads, 0, (cudaStream_t)stream>>>(
+      (__nv_bfloat16*)dqkv, ld, T, (int)n_q, (int)n_kv, (const __nv_bfloat16*)q_gamma, (const __nv_bfloat16*)k_gamma, pos,
+      inv_freq, (const __nv_bfloat16*)qk_pre, rstd, (float*)workspace);
+  PRL_LAUNCH_CHECK();
+  qk_gain_reduce_kernel<<<1, 256, 0, (cudaStream_t)stream>>>((const float*)workspace, g, dq_gamma, dk_gamma);
   PRL_LAUNCH_CHECK();
   return PRL_OK;
 }

@@ -240,6 +240,21 @@ class DecodeEngine:
                                                  x.data_ptr(), self.B if m is None else m, n, k, split,
                                                  out.data_ptr(), self._st))
 
+    def _qkv_epilogue(self, l: int, part, n_split: int, rows: int, positions, row_slot, q_out, pf_ptr, pf_bytes: int,
+                      st: int) -> None:
+        """split-K sum + bias (+ Qwen3's per-head q/k RMSNorm) + RoPE of layer l's qkv rows; q -> q_out, k / v -> KV pages"""
+        cfg, lib, a = self.cfg, self.lib, self.arena
+        p = f"layers.{l}."
+        bias = a.ptr(p + "qkv_proj.bias") if cfg.qkv_bias else None
+        slot = row_slot.data_ptr() if row_slot is not None else None
+        # without gains (Qwen2) the entry is prl_qkv_rope_cache, bit for bit
+        q_gamma, k_gamma = (a.ptr(p + "q_norm.weight"), a.ptr(p + "k_norm.weight")) if cfg.qk_norm else (None, None)
+        _lib.check(lib.prl_qkv_norm_rope_cache(part.data_ptr(), n_split, rows, bias, q_gamma, k_gamma, cfg.rms_eps,
+                                               cfg.num_q_heads, cfg.num_kv_heads, cfg.head_dim, positions.data_ptr(),
+                                               self.block_table.data_ptr(), self.max_blocks, slot, self.inv_freq.data_ptr(),
+                                               q_out.data_ptr(), self.kv_cache.data_ptr(), self.n_pages, l, PAGE_SIZE,
+                                               pf_ptr, pf_bytes, st))
+
     def _step_kernels(self) -> None:
         """Enqueue one token step for all B slots on the current stream (graph-capturable)."""
         cfg, lib, B, a = self.cfg, self.lib, self.B, self.arena
@@ -264,13 +279,8 @@ class DecodeEngine:
                 self._gemm(p + "qkv_proj.weight", self.x, cfg.qkv_size, H, self.split_k["qkv"], part)
             if "small" not in skip:
                 # while attention streams the KV cache, L2 fetches o_proj's weights
-                _lib.check(lib.prl_qkv_rope_cache(part.data_ptr(), self.split_k["qkv"], B,
-                                                  a.ptr(p + "qkv_proj.bias") if cfg.qkv_bias else None, cfg.num_q_heads,
-                                                  cfg.num_kv_heads, cfg.head_dim, self.positions.data_ptr(),
-                                                  self.block_table.data_ptr(), self.max_blocks, None,
-                                                  self.inv_freq.data_ptr(), self.q.data_ptr(), self.kv_cache.data_ptr(),
-                                                  self.n_pages, l, PAGE_SIZE,
-                                                  a.ptr(p + "o_proj.weight") if pf else None, wbytes(p + "o_proj.weight"), st))
+                self._qkv_epilogue(l, part, self.split_k["qkv"], B, self.positions, None, self.q,
+                                   a.ptr(p + "o_proj.weight") if pf else None, wbytes(p + "o_proj.weight"), st)
             if "attn" not in skip:
                 _lib.check(lib.prl_paged_attn_decode(self.q.data_ptr(), self.kv_cache.data_ptr(), self.n_pages,
                                                      cfg.num_layers, l, self.block_table.data_ptr(), self.max_blocks,
@@ -453,11 +463,7 @@ class DecodeEngine:
         for l in range(cfg.num_layers):
             p = f"layers.{l}."
             gemm(p + "qkv_proj.weight", x, cfg.qkv_size, H, part)
-            _lib.check(lib.prl_qkv_rope_cache(part.data_ptr(), 1, n, a.ptr(p + "qkv_proj.bias") if cfg.qkv_bias else None,
-                                              cfg.num_q_heads, cfg.num_kv_heads, cfg.head_dim, pf["pos"].data_ptr(),
-                                              self.block_table.data_ptr(), self.max_blocks, pf["slot"].data_ptr(),
-                                              self.inv_freq.data_ptr(), pf["q"].data_ptr(), self.kv_cache.data_ptr(),
-                                              self.n_pages, l, PAGE_SIZE, None, 0, st))
+            self._qkv_epilogue(l, part, 1, n, pf["pos"], pf["slot"], pf["q"], None, 0, st)
             seq = pf["seq"]
             if self.prefill_attn_tc:   # wgmma path (csrc/attn_tc.cu)
                 _lib.check(lib.prl_paged_attn_prefill_tc(pf["q"].data_ptr(), n, self.kv_cache.data_ptr(), self.n_pages,

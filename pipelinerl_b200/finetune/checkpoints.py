@@ -55,11 +55,23 @@ def get_temporary_folder_and_move(output_dir: Path):
 
 
 def hf_config_dict(cfg: ModelConfig) -> dict[str, Any]:
-    return {"architectures": ["Qwen2ForCausalLM"], "model_type": "qwen2", "vocab_size": cfg.vocab_size,
-            "hidden_size": cfg.hidden_size, "intermediate_size": cfg.intermediate_size, "num_hidden_layers": cfg.num_layers,
-            "num_attention_heads": cfg.num_q_heads, "num_key_value_heads": cfg.num_kv_heads, "head_dim": cfg.head_dim,
-            "hidden_act": "silu", "rms_norm_eps": cfg.rms_eps, "rope_theta": cfg.rope_theta, "tie_word_embeddings": False,
-            "torch_dtype": "bfloat16", "attention_bias": cfg.qkv_bias, "use_sliding_window": False}
+    """config.json of the checkpoint: Qwen2ForCausalLM, or Qwen3ForCausalLM for q/k-norm configs (ModelConfig.from_hf_config
+    reads it back)."""
+    if cfg.qk_norm:
+        d = {"architectures": ["Qwen3ForCausalLM"], "model_type": "qwen3"}
+    else:
+        d = {"architectures": ["Qwen2ForCausalLM"], "model_type": "qwen2"}
+    d.update({"vocab_size": cfg.vocab_size,
+              "hidden_size": cfg.hidden_size, "intermediate_size": cfg.intermediate_size, "num_hidden_layers": cfg.num_layers,
+              "num_attention_heads": cfg.num_q_heads, "num_key_value_heads": cfg.num_kv_heads, "head_dim": cfg.head_dim,
+              "hidden_act": "silu", "rms_norm_eps": cfg.rms_eps, "rope_theta": cfg.rope_theta, "tie_word_embeddings": False,
+              "torch_dtype": "bfloat16"})
+    if not cfg.qk_norm:
+        d["attention_bias"] = cfg.qkv_bias
+    elif cfg.qkv_bias:      # Qwen3Config's default is False
+        d["attention_bias"] = True
+    d["use_sliding_window"] = False
+    return d
 
 
 def _hf_tensors(cfg: ModelConfig, fused: dict[str, torch.Tensor]) -> dict[str, torch.Tensor]:

@@ -4,7 +4,7 @@ This is the part of hot path 2 that the reference runs as HF eager blocks under 
 gradient checkpointing (pipelinerl/finetune/rl/__init__.py:190-207 forward, finetune_loop.py:716-725 backward,
 conf/finetune/base.yaml:47-50 checkpointing).  Here there is no autograd inside the body:
 
-  forward   per layer: RMSNorm -> qkv GEMM(+bias) -> RoPE -> causal block-diagonal attention -> o GEMM(+residual)
+  forward   per layer: RMSNorm -> qkv GEMM(+bias) -> [Qwen3: per-head q/k RMSNorm] RoPE -> causal block-diagonal attention -> o GEMM(+residual)
             -> RMSNorm -> gate_up GEMM -> SiLU*up -> down GEMM(+residual); only each layer's INPUT is kept
   backward  per layer (reverse): recompute the MLP half (and the attention half where it was not kept), then dgrad
             GEMMs that read the weights as stored and wgrad GEMMs that read both activations as stored (MN-major
@@ -93,6 +93,29 @@ class Ops:
         T = qkv.shape[0]
         _lib.check(self.lib.prl_rope_inplace(qkv.data_ptr(), qkv.stride(0), T, n_heads, head_dim, pos.data_ptr(),
                                              inv_freq.data_ptr(), float(sign), _lib.stream_ptr()))
+
+    def qk_norm_rope_(self, qkv, pos, inv_freq, q_gamma, k_gamma, n_q, n_kv, head_dim, eps, keep):
+        """Qwen3: per-head RMSNorm (gains q_gamma / k_gamma) then RoPE of the q | k heads of qkv [T, *], in place.
+        keep: returns (pre-norm q | k columns [T, (n_q + n_kv) d] bf16, rstd [T, n_q + n_kv] fp32) for the backward."""
+        T = qkv.shape[0]
+        pre = torch.empty(T, (n_q + n_kv) * head_dim, dtype=torch.bfloat16, device=qkv.device) if keep else None
+        rstd = torch.empty(T, n_q + n_kv, dtype=torch.float32, device=qkv.device) if keep else None
+        _lib.check(self.lib.prl_qk_norm_rope_fwd(qkv.data_ptr(), qkv.stride(0), T, n_q, n_kv, head_dim, q_gamma.data_ptr(),
+                                                 k_gamma.data_ptr(), float(eps), pos.data_ptr(), inv_freq.data_ptr(),
+                                                 pre.data_ptr() if keep else None, rstd.data_ptr() if keep else None,
+                                                 _lib.stream_ptr()))
+        return (pre, rstd) if keep else None
+
+    def qk_norm_rope_bwd_(self, dqkv, pos, inv_freq, q_gamma, k_gamma, saved, n_q, n_kv, head_dim, dq_gamma, dk_gamma):
+        """in place on dqkv's q | k columns: inverse RoPE, then the RMSNorm backward; dq_gamma / dk_gamma (fp32) += gain
+        gradients (fixed reduction order)"""
+        pre, rstd = saved
+        T = dqkv.shape[0]
+        ws = torch.empty(int(self.lib.prl_rowops_workspace_bytes(256)), dtype=torch.uint8, device=dqkv.device)
+        _lib.check(self.lib.prl_qk_norm_rope_bwd(dqkv.data_ptr(), dqkv.stride(0), T, n_q, n_kv, head_dim, q_gamma.data_ptr(),
+                                                 k_gamma.data_ptr(), pos.data_ptr(), inv_freq.data_ptr(), pre.data_ptr(),
+                                                 rstd.data_ptr(), dq_gamma.data_ptr(), dk_gamma.data_ptr(), ws.data_ptr(),
+                                                 ws.numel(), _lib.stream_ptr()))
 
     def gemm_swiglu(self, x, W, need_gate_up=True):
         """(gate_up [T, 2I] or None, act [T, I]) with SiLU(gate) * up computed in the GEMM epilogue"""
@@ -284,10 +307,15 @@ class NativeBody:
         p = f"layers.{l}."
         x1, rstd1 = o.rmsnorm(h, w[p + "input_layernorm.weight"], c.rms_eps)
         qkv = o.gemm(x1, w[p + "qkv_proj.weight"], bias=w.get(p + "qkv_proj.bias"))
-        o.rope_(qkv, pos, self.inv_freq, c.num_q_heads + c.num_kv_heads, c.head_dim, +1.0)
+        qk_saved = None
+        if c.qk_norm:   # Qwen3: per-head q / k RMSNorm fused with RoPE; keeps the pre-norm q | k columns for the backward
+            qk_saved = o.qk_norm_rope_(qkv, pos, self.inv_freq, w[p + "q_norm.weight"], w[p + "k_norm.weight"],
+                                       c.num_q_heads, c.num_kv_heads, c.head_dim, c.rms_eps, keep=need_grad)
+        else:
+            o.rope_(qkv, pos, self.inv_freq, c.num_q_heads + c.num_kv_heads, c.head_dim, +1.0)
         attn, lse = self._attention(qkv, bounds, need_grad=need_grad)
         h2 = o.gemm(attn, w[p + "o_proj.weight"], residual=h)
-        return x1, rstd1, attn, (qkv, lse) if need_grad else None, h2
+        return x1, rstd1, attn, (qkv, lse, qk_saved) if need_grad else None, h2
 
     def _mlp_half(self, l, h2, need_out=True, need_gate_up=True):
         c, o, w = self.cfg, self.ops, self.w
@@ -332,8 +360,14 @@ class NativeBody:
         d_attn = o.dgrad(dh2, w[p + "o_proj.weight"])
         o.wgrad(g[p + "o_proj.weight"], dh2, attn)
         dqkv = self._attention_bwd(graph[0], attn, graph[1], bounds, d_attn)
+        qk_saved = graph[2]
         del graph, attn, d_attn
-        o.rope_(dqkv, pos, self.inv_freq, c.num_q_heads + c.num_kv_heads, c.head_dim, -1.0)
+        if c.qk_norm:
+            o.qk_norm_rope_bwd_(dqkv, pos, self.inv_freq, w[p + "q_norm.weight"], w[p + "k_norm.weight"], qk_saved,
+                                c.num_q_heads, c.num_kv_heads, c.head_dim, g[p + "q_norm.weight"], g[p + "k_norm.weight"])
+            del qk_saved
+        else:
+            o.rope_(dqkv, pos, self.inv_freq, c.num_q_heads + c.num_kv_heads, c.head_dim, -1.0)
         if c.qkv_bias:
             o.colsum_acc(dqkv, g[p + "qkv_proj.bias"])
         dx1 = o.dgrad(dqkv, w[p + "qkv_proj.weight"])

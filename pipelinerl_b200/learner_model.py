@@ -1,4 +1,4 @@
-"""Learner-side Qwen2 modules whose parameters live in the fused arena layout (model.py).
+"""Learner-side Qwen2 / Qwen3 modules whose parameters live in the fused arena layout (model.py).
 
 `NativeQwen2` (bottom of this file) is the native learner: its body is learner_body.NativeBody — hand-scheduled forward /
 backward on the wgmma GEMM and the row kernels of csrc/learner_ops.cu, fp32 gradient accumulation
@@ -24,7 +24,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
-from .model import ArenaLayout, ModelConfig, fused_shapes
+from .model import ArenaLayout, ModelConfig, fused_shapes, is_norm_gain
 
 
 class TorchQwen2(torch.nn.Module):
@@ -37,7 +37,7 @@ class TorchQwen2(torch.nn.Module):
         for name, shape in fused_shapes(cfg):
             if init is not None:
                 t = init[name].to(dtype)
-            elif name.endswith("layernorm.weight") or name == "norm.weight":
+            elif is_norm_gain(name):
                 t = torch.ones(shape, dtype=dtype)
             elif name.endswith(".bias") or name.endswith("_lo"):
                 t = torch.zeros(shape, dtype=dtype)
@@ -102,6 +102,8 @@ class TorchQwen2(torch.nn.Module):
                 q = qkv[:, :c.q_size].view(T, c.num_q_heads, c.head_dim)
                 k = qkv[:, c.q_size:c.q_size + c.kv_size].view(T, c.num_kv_heads, c.head_dim)
                 v = qkv[:, c.q_size + c.kv_size:].view(T, c.num_kv_heads, c.head_dim)
+                if c.qk_norm:   # Qwen3: per-head RMSNorm of q and k before RoPE
+                    q, k = self._norm(q, self.p(q_ + "q_norm.weight")), self._norm(k, self.p(q_ + "k_norm.weight"))
                 q, k = self._rope(q, pos), self._rope(k, pos)
                 R = c.num_q_heads // c.num_kv_heads
                 k, v = k.repeat_interleave(R, dim=1), v.repeat_interleave(R, dim=1)
@@ -214,7 +216,7 @@ class NativeQwen2(torch.nn.Module):
                 continue      # not a parameter: the bf16 residual of the head's fp32 master, kept by the optimizer (lo tail)
             if init is not None:
                 t = init[name].to(device=device, dtype=torch.bfloat16)
-            elif name.endswith("layernorm.weight") or name == "norm.weight":
+            elif is_norm_gain(name):
                 t = torch.ones(shape, dtype=torch.bfloat16, device=device)
             elif name.endswith(".bias") or name.endswith("_lo"):
                 t = torch.zeros(shape, dtype=torch.bfloat16, device=device)

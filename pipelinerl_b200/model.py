@@ -1,4 +1,4 @@
-"""Qwen2-family model description and the flat parameter arena shared by learner and sampler.
+"""Qwen2 / Qwen3 (dense) model description and the flat parameter arena shared by learner and sampler.
 
 One contiguous bf16 buffer holds every parameter in the FUSED layout the token-step kernels read
 (qkv_proj = [q; k; v] rows, gate_up_proj = [gate; up] rows).  HF parameter names
@@ -27,6 +27,7 @@ class ModelConfig:
     rope_theta: float = 1_000_000.0
     rms_eps: float = 1e-6
     qkv_bias: bool = True
+    qk_norm: bool = False    # Qwen3: per-head RMSNorm of q and k (gains q_norm / k_norm, [head_dim]) before RoPE
     fp32_head: bool = False  # keep a bf16 residual of the head (W = hi + lo): fp32-equivalent lm_head
     lm_head_rows: int | None = None  # vocabulary rows of THIS shard's lm_head (vocab-parallel head under TP)
 
@@ -76,6 +77,38 @@ class ModelConfig:
                            num_q_heads=40, num_kv_heads=8, **kw)
 
     @staticmethod
+    def qwen3_8b(**kw) -> "ModelConfig":
+        """Qwen3-8B's shapes (keyword arguments override, e.g. num_layers for a bounded sample of layers)."""
+        base = dict(vocab_size=151936, hidden_size=4096, intermediate_size=12288, num_layers=36, num_q_heads=32,
+                    num_kv_heads=8, qkv_bias=False, qk_norm=True)
+        return ModelConfig(**{**base, **kw})
+
+    @staticmethod
+    def qwen3_14b(**kw) -> "ModelConfig":
+        base = dict(vocab_size=151936, hidden_size=5120, intermediate_size=17408, num_layers=40, num_q_heads=40,
+                    num_kv_heads=8, qkv_bias=False, qk_norm=True)
+        return ModelConfig(**{**base, **kw})
+
+    @staticmethod
+    def from_hf_config(d: dict) -> "ModelConfig":
+        """ModelConfig of an HF `config.json` dict of model_type "qwen2" or "qwen3" (dense).  Tied word embeddings are
+        accepted: the arena keeps an untied copy of the head (ParamArena.load_hf_state_dict)."""
+        mt = d.get("model_type")
+        if mt not in ("qwen2", "qwen3"):
+            raise ValueError(f"unsupported model_type {mt!r}: only 'qwen2' and 'qwen3' (dense) are implemented")
+        heads = int(d["num_attention_heads"])
+        head_dim = int(d.get("head_dim") or d["hidden_size"] // heads)
+        if head_dim != 128:
+            raise ValueError(f"head_dim {head_dim} is not supported: the attention and RoPE kernels are built for 128")
+        rope = d.get("rope_parameters") or {}
+        theta = d.get("rope_theta", rope.get("rope_theta", 1_000_000.0))
+        return ModelConfig(vocab_size=int(d["vocab_size"]), hidden_size=int(d["hidden_size"]),
+                           intermediate_size=int(d["intermediate_size"]), num_layers=int(d["num_hidden_layers"]),
+                           num_q_heads=heads, num_kv_heads=int(d.get("num_key_value_heads", heads)), head_dim=head_dim,
+                           rope_theta=float(theta), rms_eps=float(d.get("rms_norm_eps", 1e-6)),
+                           qkv_bias=bool(d.get("attention_bias", mt == "qwen2")), qk_norm=mt == "qwen3")
+
+    @staticmethod
     def tiny(**kw) -> "ModelConfig":
         """Plumbing / parity-test model (config 1 of BASELINE.json is not defined by the reference)."""
         base = dict(vocab_size=512, hidden_size=256, intermediate_size=640, num_layers=2, num_q_heads=4,
@@ -94,6 +127,11 @@ def _numel(shape) -> int:
     return n
 
 
+def is_norm_gain(name: str) -> bool:
+    """RMSNorm gains (initialised to 1): the layer norms, the final norm and Qwen3's per-head q_norm / k_norm."""
+    return name.endswith("layernorm.weight") or name == "norm.weight" or name.endswith((".q_norm.weight", ".k_norm.weight"))
+
+
 def fused_shapes(cfg: ModelConfig) -> list[tuple[str, tuple[int, ...]]]:
     """Arena order.  Names are the fused (kernel-side) tensor names."""
     H, I = cfg.hidden_size, cfg.intermediate_size
@@ -104,6 +142,9 @@ def fused_shapes(cfg: ModelConfig) -> list[tuple[str, tuple[int, ...]]]:
         out.append((p + "qkv_proj.weight", (cfg.qkv_size, H)))
         if cfg.qkv_bias:
             out.append((p + "qkv_proj.bias", (cfg.qkv_size,)))
+        if cfg.qk_norm:
+            out.append((p + "q_norm.weight", (cfg.head_dim,)))
+            out.append((p + "k_norm.weight", (cfg.head_dim,)))
         out.append((p + "o_proj.weight", (H, cfg.q_size)))
         out.append((p + "post_attention_layernorm.weight", (H,)))
         out.append((p + "gate_up_proj.weight", (2 * I, H)))
@@ -146,6 +187,9 @@ class ArenaLayout:
                 m[hp + f"self_attn.q_proj.{kind}"] = (fp + f"qkv_proj.{kind}", 0, c.q_size)
                 m[hp + f"self_attn.k_proj.{kind}"] = (fp + f"qkv_proj.{kind}", c.q_size, c.kv_size)
                 m[hp + f"self_attn.v_proj.{kind}"] = (fp + f"qkv_proj.{kind}", c.q_size + c.kv_size, c.kv_size)
+            if c.qk_norm:
+                m[hp + "self_attn.q_norm.weight"] = (fp + "q_norm.weight", 0, c.head_dim)
+                m[hp + "self_attn.k_norm.weight"] = (fp + "k_norm.weight", 0, c.head_dim)
             m[hp + "self_attn.o_proj.weight"] = (fp + "o_proj.weight", 0, c.hidden_size)
             m[hp + "mlp.gate_proj.weight"] = (fp + "gate_up_proj.weight", 0, c.intermediate_size)
             m[hp + "mlp.up_proj.weight"] = (fp + "gate_up_proj.weight", c.intermediate_size, c.intermediate_size)
@@ -182,11 +226,12 @@ class ParamArena:
         return self.data.numel() * self.data.element_size()
 
     def init_random(self, seed: int = 42, std: float = 0.02) -> "ParamArena":
-        """normal(0, 0.02) weights, unit norm gains, zero biases — HF's Qwen2 initialisation; seed = conf/base.yaml:7."""
+        """normal(0, 0.02) weights, unit norm gains (q_norm / k_norm included), zero biases — HF's Qwen2 / Qwen3
+        initialisation; seed = conf/base.yaml:7."""
         g = torch.Generator(device=self.data.device).manual_seed(seed)
         for name in self.names():
             v = self.view(name)
-            if name.endswith("layernorm.weight") or name == "norm.weight":
+            if is_norm_gain(name):
                 v.fill_(1.0)
             elif name.endswith(".bias") or name.endswith("_lo"):
                 v.zero_()

@@ -33,6 +33,9 @@ class TPDecodeEngine(DecodeEngine):
 
     def __init__(self, full_cfg: ModelConfig, arena: ParamArena, tp_rank: int, tp_size: int, group=None, **kw):
         import torch.distributed as dist
+        if full_cfg.qk_norm:
+            raise NotImplementedError("TPDecodeEngine does not implement Qwen3's q/k norm yet (qk_norm=True): "
+                                      "use DecodeEngine")
         if tp_size < 2 or tp_size > 8:
             raise ValueError("TPDecodeEngine is for 2..8 ranks; use DecodeEngine for tp=1")
         self.full_cfg, self.tp_rank, self.tp, self.dist, self.group = full_cfg, tp_rank, tp_size, dist, group
