@@ -285,7 +285,8 @@ int prl_preprocess_pack(const prl_mb_record* record, int32_t divide_advantage_by
  *   splits in index order (deterministic).  K %% 8 == 0; pointers 16-B aligned.
  * ======================================================================= */
 int prl_gemm_auto_split_k(int64_t M, int64_t N, int64_t K);
-/* Tuning knob: shared-memory tile ring per CTA in KB (<= 100 lets two CTAs share an SM). */
+/* Tuning knob: shared-memory tile ring per CTA in KB at <= 64 tokens (default 72: three CTAs share an SM; <= 100: two).
+ * The ring depth never changes results. */
 int prl_gemm_set_smem_budget_kb(int32_t kb);
 /* Weight layout switch: 0 = row-major [N,K]; 1 = contiguous 16 KB tiles [N/128][K/64][128][64] (one sequential
  * TMA box per tile; needs N % 128 == 0, K % 64 == 0). */

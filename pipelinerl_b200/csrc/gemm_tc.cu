@@ -106,8 +106,12 @@ constexpr int kBlockM = 128;  // output features per CTA (two wgmma M = 64 halve
 constexpr int kBlockK = 64;   // bf16 elements per stage row = 128 B = one swizzle atom
 constexpr int kUmmaK = 16;
 constexpr int kThreads = 288;
-static int g_smem_budget = 100 * 1024;
-static int g_tiled_weights = 0;  // weights stored as contiguous [N/128][K/64][128][64] tiles  // per-CTA tile ring; <= 100 KB lets two CTAs share an SM
+// Per-CTA tile ring at kNTile <= 64.  72 KB = 3 stages at the decode batch (kNTile = 64, 24 KB per stage) lets THREE CTAs
+// share an SM (the kernel needs fewer than 75 registers per thread), so the token step's split plans (qkv 36 x 11 = 396,
+// o and down 28 x 14 = 392, gate_up 296 CTAs) each run as one wave on 132 SMs instead of 1.1-1.5 waves with two CTAs
+// per SM and a 96 KB ring.  The ring depth does not change any CTA's k-range: results are the same bits.
+static int g_smem_budget = 72 * 1024;
+static int g_tiled_weights = 0;  // weights stored as contiguous [N/128][K/64][128][64] tiles
 
 struct HeadPart { float m, s, u, key, z; int idx; };  // per (vocab tile, token): online-softmax state + best sample
 

@@ -39,7 +39,7 @@ def main():
         W = (torch.randn(N, K, device=dev) * 0.02).to(torch.bfloat16)
         X = torch.randn(B, K, device=dev).to(torch.bfloat16)
         auto = lib.prl_gemm_auto_split_k(B, N, K)
-        for budget, tiled in ((100, 0), (100, 1), (200, 1)):
+        for budget, tiled in ((72, 0), (100, 0), (100, 1), (200, 1)):
             lib.prl_gemm_set_smem_budget_kb(budget)
             lib.prl_gemm_set_tiled_weights(tiled)   # timing experiment: tiled addressing of the same buffer
             for split in sorted(set([auto, auto * 2])):
@@ -53,7 +53,7 @@ def main():
                             "auto": auto, "us": round(us, 2), "weight_GBs": round(gbs, 1)})
                 print(json.dumps(out[-1]), flush=True)
         del W
-    lib.prl_gemm_set_smem_budget_kb(100)
+    lib.prl_gemm_set_smem_budget_kb(72)   # the library default
     lib.prl_gemm_set_tiled_weights(0)
     # epilogue kernels
     h = torch.randn(B, H, device=dev)

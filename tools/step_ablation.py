@@ -19,13 +19,15 @@ def main():
     from pipelinerl_b200 import _lib
     lib = _lib.load()
     # (name, skipped kernel classes, L2 prefetch bytes, fused head, PDL, fused attention combine, gemm smem KB)
-    variants = [("base", set(), 0, True, 1, 0, 100), ("base_again", set(), 0, True, 1, 0, 100),
-                ("fused_combine", set(), 0, True, 1, 1, 100), ("no_pdl", set(), 0, True, 0, 0, 100),
-                ("unfused_head", set(), 0, False, 1, 0, 100), ("gemm_smem_200", set(), 0, True, 1, 0, 200),
-                ("gemm_smem_72", set(), 0, True, 1, 0, 72), ("l2_prefetch_40MB", set(), 40 << 20, True, 1, 0, 100),
-                ("no_attention", {"attn"}, 0, True, 1, 0, 100), ("gemm_only", {"attn", "small"}, 0, True, 1, 0, 100),
-                ("attention_only", {"gemm", "small"}, 0, True, 1, 0, 100), ("small_only", {"gemm", "attn"}, 0, True, 1, 0, 100),
-                ("base_end", set(), 0, True, 1, 0, 100)]
+    # gemm smem 72 KB is the library default (three GEMM CTAs per SM); 100 KB = two, 48 KB = 2-stage rings
+    variants = [("base", set(), 0, True, 1, 0, 72), ("base_again", set(), 0, True, 1, 0, 72),
+                ("fused_combine", set(), 0, True, 1, 1, 72), ("no_pdl", set(), 0, True, 0, 0, 72),
+                ("unfused_head", set(), 0, False, 1, 0, 72), ("gemm_smem_200", set(), 0, True, 1, 0, 200),
+                ("gemm_smem_100", set(), 0, True, 1, 0, 100), ("gemm_smem_48", set(), 0, True, 1, 0, 48),
+                ("l2_prefetch_40MB", set(), 40 << 20, True, 1, 0, 72),
+                ("no_attention", {"attn"}, 0, True, 1, 0, 72), ("gemm_only", {"attn", "small"}, 0, True, 1, 0, 72),
+                ("attention_only", {"gemm", "small"}, 0, True, 1, 0, 72), ("small_only", {"gemm", "attn"}, 0, True, 1, 0, 72),
+                ("base_end", set(), 0, True, 1, 0, 72)]
     for name, skip, pf, fused, pdl, fcomb, smem in variants:
         eng._skip, eng.l2_prefetch_bytes, eng.fused_head = skip, pf, fused
         lib.prl_set_pdl(pdl)
