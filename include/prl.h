@@ -531,7 +531,10 @@ int prl_sample_logprob_topkp_rows(const float* logits /*[B,V]*/, int32_t B, int3
  * prl_advance_state moves every active slot one token forward without a host round trip:
  * feeds the next prompt token while inside the prompt, else appends (sampled id, logprob) to the
  * slot's output ring, and retires the slot on EOS (finished=1, "stop") or max_new (finished=2, "length")
- * — the finish_reason values pipelinerl/async_llm.py:202-212 reports. */
+ * — the finish_reason values pipelinerl/async_llm.py:202-212 reports.
+ * The checks run in vLLM's check_stop order after the id is appended (a stop token stays in the output with its
+ * logprob): the primary eos_id unless the slot ignores eos, then membership in the slot's stop row, then the length
+ * cap.  With stop_ids == NULL the stop row is skipped and every other field behaves exactly as without it. */
 typedef struct {
   int32_t B;
   const int32_t* sampled;          /* [B] ids drawn by prl_sample_logprob this step */
@@ -552,6 +555,13 @@ typedef struct {
   int32_t eos_id;
   int32_t ignore_eos;              /* engine-wide: never stop on eos */
   const uint8_t* ignore_eos_rows;  /* [B] per sequence (may be NULL) */
+  /* extra stop ids per slot (generation_config's other eos ids, request stop_token_ids); checked whatever the slot's
+   * ignore_eos says, so a caller drops the generation_config ids from the row of an ignore_eos request */
+  const int32_t* stop_ids;         /* [B, stop_stride] or NULL: no stop sets */
+  int32_t stop_stride;
+  const int32_t* n_stop;           /* [B] ids used in each row (0..stop_stride); required with stop_ids */
+  int32_t* stop_reason;            /* [B] or NULL; written when a slot finishes: the stop-row id that matched, else -1
+                                      (primary eos or length) */
 } prl_engine_state;
 int prl_advance_state(const prl_engine_state* state, prl_stream_t stream);
 

@@ -76,6 +76,7 @@ class EngineState(C.Structure):
         ("prompt_stride", C.c_int32), ("prompt_len", C.c_void_p), ("out_ids", C.c_void_p),
         ("out_logprobs", C.c_void_p), ("out_stride", C.c_int32), ("gen_count", C.c_void_p), ("max_new", C.c_void_p),
         ("finished", C.c_void_p), ("eos_id", C.c_int32), ("ignore_eos", C.c_int32), ("ignore_eos_rows", C.c_void_p),
+        ("stop_ids", C.c_void_p), ("stop_stride", C.c_int32), ("n_stop", C.c_void_p), ("stop_reason", C.c_void_p),
     ]
 
 

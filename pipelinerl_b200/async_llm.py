@@ -2,7 +2,7 @@
 (reference: pipelinerl/async_llm.py:86-212 and :215-346)."""
 from __future__ import annotations
 
-from .engine import SamplingParams, requested_truncation, truncation_params
+from .engine import SamplingParams, requested_truncation, stop_token_ids_param, truncation_params
 from .llm import LLMCall, LLMOutput, Prompt, TokenLogprob, TrainableLLM
 from .rollouts import TrainingText, apply_rollout_reward
 from .serving import resolve, sampling_features
@@ -34,25 +34,29 @@ def _chat_kwargs(llm: TrainableLLM, prompt: Prompt) -> dict:
     return kw
 
 
-def _reject_unsupported_sampling(params: dict, features: frozenset = frozenset()) -> tuple[int, float]:
+def _reject_unsupported_sampling(params: dict, features: frozenset = frozenset()) -> tuple[int, float, tuple[int, ...]]:
     """Sampling features the engine does not implement must fail loudly, exactly as http_shim.py answers 400 for them:
     a silently ignored top_p / top_k / stop would make the recorded logprobs those of a different distribution than the
     one the request asked for.  top_k / top_p are accepted when the target engine lists them in `features` (the unfused
-    single-GPU DecodeEngine does; the reference's eval handles send top_p 0.95 / top_k 50, conf/base.yaml:52-57); they
-    are validated as vLLM validates them.  Returns the request's (top_k, top_p)."""
+    single-GPU DecodeEngine does; the reference's eval handles send top_p 0.95 / top_k 50, conf/base.yaml:52-57), and
+    stop_token_ids when it lists "stop_token_ids"; they are validated as vLLM validates them.  Stop strings are refused.
+    Returns the request's (top_k, top_p, stop_token_ids)."""
     greedy = float(params.get("temperature", 1.0)) <= 0
     top_k, top_p = truncation_params(params, greedy=greedy)
     missing = requested_truncation(top_k, top_p) - features
     if missing:
         raise ValueError(f"{' / '.join(sorted(missing))} sampling is not implemented by this engine")
-    if params.get("stop") or params.get("stop_token_ids"):
-        raise ValueError("stop strings / stop token ids are not implemented by this engine (eos only)")
+    stop_ids = stop_token_ids_param(params)
+    if stop_ids and "stop_token_ids" not in features:
+        raise ValueError("stop token ids are not implemented by this engine (eos only)")
+    if params.get("stop"):
+        raise ValueError("stop strings are not implemented by this engine (stop token ids are)")
     if int(params.get("n", 1)) != 1:
         raise ValueError("n > 1 completions per request is not implemented (the actor issues `attempts` requests)")
     for name in ("presence_penalty", "frequency_penalty", "repetition_penalty", "min_p"):
         if params.get(name) not in (None, 0, 0.0, 1, 1.0) or (name == "repetition_penalty" and params.get(name) not in (None, 1, 1.0)):
             raise ValueError(f"sampling parameter {name} is not implemented by this engine")
-    return top_k, top_p
+    return top_k, top_p, stop_ids
 
 
 async def llm_async_generate(llm: TrainableLLM, prompt: Prompt, session=None,
@@ -64,18 +68,22 @@ async def llm_async_generate(llm: TrainableLLM, prompt: Prompt, session=None,
     prompt_ids = prompt.token_ids or _token_ids(tok.apply_chat_template(prompt.messages, add_generation_prompt=True,
                                                                         **_chat_kwargs(llm, prompt)))
     params = llm.parameters
-    top_k, top_p = _reject_unsupported_sampling(params, sampling_features(llm.base_url))
+    top_k, top_p, stop_ids = _reject_unsupported_sampling(params, sampling_features(llm.base_url))
     max_tokens = int(max_tokens_override if max_tokens_override is not None else params.get("max_tokens", 16))
     temperature = float(params.get("temperature", 1.0))
     sp = SamplingParams(max_tokens=max_tokens, temperature=temperature if temperature > 0 else 1.0,
                         greedy=temperature <= 0, ignore_eos=bool(params.get("ignore_eos", False)), top_k=top_k,
-                        top_p=top_p)
-    req = await resolve(llm.base_url).generate(list(prompt_ids), sp)
+                        top_p=top_p, stop_token_ids=stop_ids)
+    server = resolve(llm.base_url)
+    if stop_ids:
+        server.engine.stop_row(sp)      # out-of-vocabulary ids or too many: ValueError here, not on the engine thread
+    req = await server.generate(list(prompt_ids), sp)
     content = tok.decode(req.output_ids)
     call = llm.log_output(prompt, LLMOutput(content=content), count_tokens=False)
     call.prompt_length_tokens = len(prompt_ids)
     call.output_length_tokens = len(req.output_ids)
     call.llm_info["finish_reason"] = req.finish_reason
+    call.llm_info["stop_reason"] = getattr(req, "stop_reason", None)
     call.llm_info["model_version"] = req.model_version
     call.llm_info["prompt_token_ids"] = list(prompt_ids)
     if llm.collect_logprobs:

@@ -479,8 +479,24 @@ __global__ void advance_kernel(prl_engine_state st) {
     st.tokens[b] = id;
     const bool ignore = st.ignore_eos || (st.ignore_eos_rows != nullptr && st.ignore_eos_rows[b]);
     const bool eos = (id == st.eos_id) && !ignore;
-    if (eos || n + 1 >= st.max_new[b]) {
-      st.finished[b] = eos ? 1 : 2;  // 1 = stop, 2 = length
+    // vLLM's check_stop order: the primary eos, then the slot's stop set, then the length cap, so a stop id drawn as
+    // the last allowed token reports "stop"
+    bool stop = eos;
+    int reason = -1;
+    if (!eos && st.stop_ids != nullptr) {
+      const int32_t* row = st.stop_ids + (int64_t)b * st.stop_stride;
+      const int m = min(st.n_stop[b], st.stop_stride);
+      for (int j = 0; j < m; ++j) {
+        if (row[j] == id) {
+          stop = true;
+          reason = id;
+          break;
+        }
+      }
+    }
+    if (stop || n + 1 >= st.max_new[b]) {
+      st.finished[b] = stop ? 1 : 2;  // 1 = stop, 2 = length
+      if (st.stop_reason != nullptr) st.stop_reason[b] = reason;
       st.active[b] = 0;
       st.seq_lens[b] = 0;            // the slot stops reading its KV
       st.positions[b] = 0;
@@ -652,6 +668,8 @@ extern "C" int prl_advance_state(const prl_engine_state* state, prl_stream_t st)
                     state->active && state->prompt_buf && state->prompt_len && state->out_ids &&
                     state->out_logprobs && state->gen_count && state->max_new && state->finished,
                 "prl_advance_state: NULL field");
+  PRL_CHECK_ARG(state->stop_ids == nullptr || (state->n_stop && state->stop_stride >= 1),
+                "prl_advance_state: stop_ids needs n_stop and stop_stride >= 1");
   PRL_CUDA(launch_pdl(advance_kernel, dim3((state->B + 127) / 128), dim3(128), 0, (cudaStream_t)st, *state));
   PRL_LAUNCH_CHECK();
   return PRL_OK;

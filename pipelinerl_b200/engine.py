@@ -21,7 +21,7 @@ from dataclasses import dataclass, field
 import torch
 
 from . import _lib
-from .model import ModelConfig, ParamArena
+from .model import ModelConfig, ParamArena, rope_inv_freq
 
 PAGE_SIZE = 64
 
@@ -34,6 +34,7 @@ class SamplingParams:
     ignore_eos: bool = False
     top_k: int = -1          # -1 / 0: off; 1 <= k < vocabulary: keep the k largest logits (and every tie of the k-th)
     top_p: float = 1.0       # 1: off; else keep the smallest top set holding mass >= top_p (vLLM's rule)
+    stop_token_ids: tuple[int, ...] = ()   # ids that end the request with finish_reason "stop", even with ignore_eos
 
 
 def truncation_params(params: dict, greedy: bool = False) -> tuple[int, float]:
@@ -54,6 +55,28 @@ def truncation_params(params: dict, greedy: bool = False) -> tuple[int, float]:
     return int(top_k), float(top_p)
 
 
+def stop_token_ids_param(params: dict) -> tuple[int, ...]:
+    """`stop_token_ids` of a request body / `llm.parameters`, validated as vLLM validates it (a list of integers; a
+    missing or None value is empty).  Raises ValueError."""
+    ids = params.get("stop_token_ids")
+    if ids is None:
+        return ()
+    if not isinstance(ids, (list, tuple)) or any(isinstance(t, bool) or not isinstance(t, int) for t in ids):
+        raise ValueError(f"stop_token_ids must contain only integers, got {ids!r}")
+    return tuple(ids)
+
+
+def stop_ids_from_generation_config(gen_cfg: dict, eos_token_id: int | None) -> tuple[int, tuple[int, ...]]:
+    """(eos_id, stop_ids) for DecodeEngine from a `generation_config.json` dict and the tokenizer's eos id, as vLLM's
+    SamplingParams.update_from_generation_config splits them: the tokenizer's eos is the primary eos (-1: none), and
+    every other id generation_config lists as `eos_token_id` is an extra stop id (dropped by ignore_eos requests)."""
+    ids = gen_cfg.get("eos_token_id")
+    ids = set() if ids is None else {ids} if isinstance(ids, int) else set(ids)
+    if eos_token_id is not None:
+        ids.discard(eos_token_id)
+    return (-1 if eos_token_id is None else int(eos_token_id)), tuple(sorted(int(i) for i in ids))
+
+
 def requested_truncation(top_k: int, top_p: float) -> set[str]:
     """The truncation features a validated (top_k, top_p) pair asks for."""
     return ({"top_k"} if top_k > 0 else set()) | ({"top_p"} if top_p < 1.0 else set())
@@ -69,6 +92,7 @@ class Request:
     output_ids: list[int] = field(default_factory=list)
     output_logprobs: list[float] = field(default_factory=list)
     finish_reason: str | None = None
+    stop_reason: int | None = None                       # the stop id that ended it (vLLM's stop_reason); None for eos / length
     model_version: int = 0
     prefilled: int = 0                                   # prompt tokens whose KV is in the cache
     waits_for: list = field(default_factory=list)        # [(request filling a shared page, tokens it must reach)]
@@ -78,7 +102,7 @@ class DecodeEngine:
     def __init__(self, cfg: ModelConfig, arena: ParamArena, max_batch: int = 64, max_seq_len: int = 16384,
                  n_pages: int | None = None, max_new_tokens: int = 8192, eos_id: int = -1, seed: int = 42,
                  device: torch.device | str = "cuda:0", use_cuda_graph: bool = True, prefill_chunk: int = 1024,
-                 prefix_sharing: bool = True, fused_head: bool = False):
+                 prefix_sharing: bool = True, fused_head: bool = False, stop_ids=(), max_stop_ids: int = 16):
         if cfg.head_dim != 128:
             raise ValueError("the sm_90a attention kernel is built for head_dim 128")
         self.cfg, self.arena = cfg, arena
@@ -93,6 +117,14 @@ class DecodeEngine:
         self.n_pages = n_pages if n_pages is not None else 1 + self.B * self.max_blocks
         self.max_new = max_new_tokens
         self.eos_id, self.seed = eos_id, seed
+        # generation_config's extra eos ids (stop_ids_from_generation_config): every request that does not ignore eos
+        # stops on them as well
+        self.max_stop_ids = int(max_stop_ids)
+        self.stop_ids = tuple(int(t) for t in stop_ids)
+        if self.max_stop_ids < 1 or len(set(self.stop_ids)) > self.max_stop_ids:
+            raise ValueError(f"{len(set(self.stop_ids))} engine stop ids do not fit rows of max_stop_ids={max_stop_ids}")
+        if self.stop_ids:
+            self._check_token_ids(self.stop_ids)
         self.use_graph = use_cuda_graph
         # fused_head: lm_head + sampling + logprob capture in one GEMM epilogue (no logits in HBM).  For the 64-row
         # decode step the logits round trip is only 78 MB and the fused epilogue cannot live in the step's CUDA graph
@@ -130,9 +162,7 @@ class DecodeEngine:
         self.attn_out = torch.zeros(B, cfg.q_size, dtype=torch.bfloat16, device=d)
         self.act = torch.zeros(B, I, dtype=torch.bfloat16, device=d)
         self.logits = torch.zeros(B, cfg.head_rows, dtype=torch.float32, device=d)
-        # HF rotary: inv_freq = 1 / theta^(arange(0, d, 2) / d) in fp32
-        self.inv_freq = (1.0 / (cfg.rope_theta ** (torch.arange(0, cfg.head_dim, 2, dtype=torch.int64).float()
-                                                   / cfg.head_dim))).to(d)
+        self.inv_freq = rope_inv_freq(cfg).to(d)
         self._plan_gemms()
         self.attn_splits = int(self.lib.prl_paged_attn_splits(B, cfg.num_kv_heads, max_seq_len))
         self.attn_ws = torch.zeros(int(self.lib.prl_paged_attn_workspace_bytes(B, cfg.num_q_heads, self.attn_splits)),
@@ -154,6 +184,12 @@ class DecodeEngine:
         self.top_k_rows = torch.full((B,), -1, dtype=torch.int32, device=d)
         self.top_p_rows = torch.ones(B, dtype=torch.float32, device=d)
         self._truncated_slots: set[int] = set()
+        # stop sets per slot; the advance kernel gets them only while some slot in _stop_slots has a non-empty row, so
+        # without stop ids it runs exactly as it did before stop sets existed
+        self.stop_rows = torch.zeros(B, self.max_stop_ids, dtype=torch.int32, device=d)
+        self.n_stop = torch.zeros(B, dtype=torch.int32, device=d)
+        self.stop_reason = torch.full((B,), -1, dtype=torch.int32, device=d)
+        self._stop_slots: set[int] = set()
         self._temperature, self._greedy, self._ignore_eos = 1.0, False, False
         self._graphs: dict[int, torch.cuda.CUDAGraph] = {}
         # ---- chunked prefill + prefix sharing (GRPO attempts share their prompt) ----
@@ -178,6 +214,10 @@ class DecodeEngine:
         """Truncation this engine samples with (`add_request` refuses the rest): the unfused sampler implements top-k and
         top-p; the fused sampling head does not."""
         return frozenset() if self.fused_head else frozenset({"top_k", "top_p"})
+
+    # per-request stop_token_ids: the state advance checks each slot's stop set, so every engine that calls
+    # prl_advance_state (fused head and TP included) has them; clients read this before sending stop ids
+    supports_stop_token_ids = True
 
     # engine-wide sampling defaults: assigning one overwrites every slot (benches, tools, single-tenant tests)
     @property
@@ -231,7 +271,14 @@ class DecodeEngine:
         s.gen_count, s.max_new, s.finished = self.gen_count.data_ptr(), self.max_new_t.data_ptr(), self.finished.data_ptr()
         s.eos_id, s.ignore_eos = self.eos_id, 0
         s.ignore_eos_rows = self.ignore_eos_rows.data_ptr()
+        s.stop_stride, s.n_stop = self.max_stop_ids, self.n_stop.data_ptr()
         return s
+
+    def _advance(self, st: int) -> None:
+        on = bool(self._stop_slots)
+        self._state.stop_ids = self.stop_rows.data_ptr() if on else None
+        self._state.stop_reason = self.stop_reason.data_ptr() if on else None
+        _lib.check(self.lib.prl_advance_state(C.byref(self._state), st))
 
     # ------------------------------------------------------------------------------------------
     def _gemm(self, w_name: str, x: torch.Tensor, n: int, k: int, split: int, out: torch.Tensor, lo: str | None = None,
@@ -330,7 +377,7 @@ class DecodeEngine:
                                             float(self.temperature), None, int(self.greedy), self.seed, self.step_count,
                                             None, None, None, self.sampled.data_ptr(), self.sampled_lp.data_ptr(),
                                             self.head_ws.data_ptr(), self.head_ws.numel(), st))
-            _lib.check(lib.prl_advance_state(C.byref(self._state), st))
+            self._advance(st)
             return
         if self._truncated_slots:
             _lib.check(lib.prl_sample_logprob_topkp_rows(self.logits.data_ptr(), self.B, self.cfg.head_rows,
@@ -344,7 +391,7 @@ class DecodeEngine:
                                                    self.inv_temp_rows.data_ptr(), self.greedy_rows.data_ptr(), self.seed,
                                                    self.step_count, self.sampled.data_ptr(), self.sampled_lp.data_ptr(),
                                                    self.sample_ws.data_ptr(), self.sample_ws.numel(), st))
-        _lib.check(lib.prl_advance_state(C.byref(self._state), st))
+        self._advance(st)
 
     def step(self) -> None:
         """One token for every active slot.  The model part is replayed from a CUDA graph; sampling and
@@ -403,6 +450,19 @@ class DecodeEngine:
         lo, hi = min(ids), max(ids)
         if lo < 0 or hi >= self.cfg.vocab_size:
             raise ValueError(f"token id out of range [0, {self.cfg.vocab_size}): min {lo}, max {hi}")
+
+    def stop_row(self, params: SamplingParams) -> list[int]:
+        """The slot's stop set for a request: its own stop_token_ids, plus the engine's stop_ids unless it ignores eos
+        (vLLM's rule: ignore_eos drops generation_config's extra eos ids, not the request's own).  Raises ValueError for
+        ids outside the vocabulary or more distinct ids than a row holds."""
+        own = stop_token_ids_param({"stop_token_ids": params.stop_token_ids})
+        if own:
+            self._check_token_ids(own)
+        ids = own if (params.ignore_eos or self._ignore_eos) else own + self.stop_ids
+        row = list(dict.fromkeys(ids))
+        if len(row) > self.max_stop_ids:
+            raise ValueError(f"{len(row)} stop token ids exceed this engine's limit of {self.max_stop_ids}")
+        return row
 
     # ---- chunked prefill ------------------------------------------------------------------------
     def _prefill_buffers(self):
@@ -632,6 +692,7 @@ class DecodeEngine:
         if missing:
             raise ValueError(f"{' / '.join(sorted(missing))} sampling is not implemented by this engine "
                              f"({type(self).__name__}, fused_head={self.fused_head})")
+        stop = self.stop_row(params)
         if not self.can_admit(n, params.max_tokens):
             raise RuntimeError("engine full")
         req = Request(self._next_id, list(prompt_ids), params, model_version=model_version)
@@ -689,6 +750,10 @@ class DecodeEngine:
         if requested_truncation(top_k, top_p):
             self._truncated_slots.add(slot)
         self.ignore_eos_rows[slot] = int(bool(params.ignore_eos) or self._ignore_eos)
+        if stop:                                   # rows of other slots keep n_stop 0 (reset at harvest)
+            self.n_stop[slot] = len(stop)
+            self.stop_rows[slot, :len(stop)].copy_(torch.tensor(stop, dtype=torch.int32), non_blocking=True)
+            self._stop_slots.add(slot)
         self.tokens[slot] = prompt_ids[start]
         self.positions[slot] = start
         self.seq_lens[slot] = start + 1
@@ -703,6 +768,7 @@ class DecodeEngine:
         if not self.slot_req:
             return []
         fin = self.finished.cpu()
+        reason = self.stop_reason.cpu() if self._stop_slots else None
         done = []
         for slot, req in list(self.slot_req.items()):
             code = int(fin[slot])
@@ -712,6 +778,10 @@ class DecodeEngine:
             req.output_ids = self.out_ids[slot, :n].cpu().tolist()
             req.output_logprobs = self.out_logprobs[slot, :n].cpu().tolist()
             req.finish_reason = "stop" if code == 1 else "length"
+            if slot in self._stop_slots:
+                self._stop_slots.discard(slot)
+                self.n_stop[slot] = 0
+                req.stop_reason = int(reason[slot]) if code == 1 and int(reason[slot]) >= 0 else None
             self.block_table[slot].zero_()
             self.finished[slot] = 0
             if slot in self._truncated_slots:

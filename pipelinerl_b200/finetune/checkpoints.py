@@ -55,8 +55,16 @@ def get_temporary_folder_and_move(output_dir: Path):
 
 
 def hf_config_dict(cfg: ModelConfig) -> dict[str, Any]:
-    """config.json of the checkpoint: Qwen2ForCausalLM, or Qwen3ForCausalLM for q/k-norm configs (ModelConfig.from_hf_config
-    reads it back)."""
+    """config.json of the checkpoint: Qwen2ForCausalLM, Qwen3ForCausalLM for q/k-norm configs, or LlamaForCausalLM
+    (ModelConfig.from_hf_config reads it back)."""
+    if cfg.family == "llama":
+        return {"architectures": ["LlamaForCausalLM"], "model_type": "llama", "vocab_size": cfg.vocab_size,
+                "hidden_size": cfg.hidden_size, "intermediate_size": cfg.intermediate_size,
+                "num_hidden_layers": cfg.num_layers, "num_attention_heads": cfg.num_q_heads,
+                "num_key_value_heads": cfg.num_kv_heads, "head_dim": cfg.head_dim, "hidden_act": "silu",
+                "rms_norm_eps": cfg.rms_eps, "rope_theta": cfg.rope_theta,
+                "rope_scaling": cfg.rope_scaling.hf_dict() if cfg.rope_scaling is not None else None,
+                "tie_word_embeddings": False, "torch_dtype": "bfloat16", "attention_bias": False, "mlp_bias": False}
     if cfg.qk_norm:
         d = {"architectures": ["Qwen3ForCausalLM"], "model_type": "qwen3"}
     else:

@@ -18,7 +18,9 @@ at this shim instead of a vLLM server (SURVEY §8b "wire format"):
                               the learner's P2P push; the endpoint only reports the version the sampler is serving.
 
 top_k / top_p are served when the engine lists them in `engine.sampling_features` (the unfused single-GPU DecodeEngine:
-vLLM's truncation rule, with the logprob of the truncated distribution) and are validated as vLLM validates them.
+vLLM's truncation rule, with the logprob of the truncated distribution), and stop_token_ids when the engine sets
+`supports_stop_token_ids` (every DecodeEngine; the choice then reports vLLM's `stop_reason`, the stop id that ended it).
+They are validated as vLLM validates them.
 Sampling features the engine does not implement (truncation on the fused-head or TP engines, n > 1, streaming) are
 rejected with 400 rather than silently ignored.  Host code only: the engine behind it is the CUDA DecodeEngine (no CPU
 fallback).
@@ -33,7 +35,8 @@ from typing import Any
 
 from aiohttp import web
 
-from .engine import SamplingParams, requested_truncation, truncation_params
+from .engine import SamplingParams, requested_truncation, stop_token_ids_param, truncation_params
+from .serving import engine_features
 
 
 def _token_ids(encoded) -> list[int]:
@@ -109,17 +112,27 @@ class HttpShim:
         temperature = float(body.get("temperature", 1.0))
         try:
             top_k, top_p = truncation_params(body, greedy=temperature <= 0)
+            stop_ids = stop_token_ids_param(body)
         except ValueError as e:
             return self._bad(str(e))
         engine = getattr(self.server, "engine", None)
-        missing = requested_truncation(top_k, top_p) - frozenset(getattr(engine, "sampling_features", frozenset()))
+        features = engine_features(engine)
+        missing = requested_truncation(top_k, top_p) - features
         if missing:
             return self._bad(f"{' / '.join(sorted(missing))} sampling is not implemented by this engine")
+        if stop_ids and "stop_token_ids" not in features:
+            return self._bad("stop_token_ids are not implemented by this engine")
         if int(body.get("n", 1)) != 1 or body.get("stream"):
             return self._bad("n > 1 and streaming are not implemented")
         max_tokens = int(body.get("max_tokens") or body.get("max_completion_tokens") or self.default_max_tokens)
-        return SamplingParams(max_tokens=max_tokens, temperature=temperature if temperature > 0 else 1.0,
-                              greedy=temperature <= 0, top_k=top_k, top_p=top_p)
+        sp = SamplingParams(max_tokens=max_tokens, temperature=temperature if temperature > 0 else 1.0,
+                            greedy=temperature <= 0, top_k=top_k, top_p=top_p, stop_token_ids=stop_ids)
+        if stop_ids:
+            try:
+                engine.stop_row(sp)        # ids outside the vocabulary, or more than a slot's stop row holds
+            except ValueError as e:
+                return self._bad(str(e))
+        return sp
 
     async def chat_completions(self, request: web.Request) -> web.Response:
         body = await request.json()
@@ -138,7 +151,7 @@ class HttpShim:
         # include_stop_str_in_output / skip_special_tokens=False (what the reference asks for): decode every id
         content = self._decode(out_ids)
         choice: dict[str, Any] = {"index": 0, "message": {"role": "assistant", "content": content, "tool_calls": []},
-                                  "finish_reason": req.finish_reason, "stop_reason": None}
+                                  "finish_reason": req.finish_reason, "stop_reason": getattr(req, "stop_reason", None)}
         if body.get("logprobs"):
             choice["logprobs"] = {"content": [{"token": f"token_id:{t}", "logprob": float(lp), "bytes": None,
                                                "top_logprobs": []} for t, lp in zip(out_ids, req.output_logprobs)]}

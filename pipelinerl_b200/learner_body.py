@@ -22,7 +22,7 @@ import math
 import torch
 
 from . import _lib
-from .model import ModelConfig
+from .model import ModelConfig, rope_inv_freq
 
 
 def _ru(x: int, m: int) -> int:
@@ -232,8 +232,7 @@ class NativeBody:
         self.cfg, self.w, self.g = cfg, weights, grads
         self.ops = Ops()
         dev = next(iter(weights.values())).device
-        d = cfg.head_dim
-        self.inv_freq = (1.0 / (cfg.rope_theta ** (torch.arange(0, d, 2, dtype=torch.int64).float() / d))).to(dev)
+        self.inv_freq = rope_inv_freq(cfg).to(dev)
         self._saved = None
         self._seg_cache = None
         self.keep_attention_layers = cfg.num_layers   # lower it when activation memory is short (0 = full recompute)

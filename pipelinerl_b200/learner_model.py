@@ -24,7 +24,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
-from .model import ArenaLayout, ModelConfig, fused_shapes, is_norm_gain
+from .model import ArenaLayout, ModelConfig, fused_shapes, is_norm_gain, rope_inv_freq
 
 
 class TorchQwen2(torch.nn.Module):
@@ -46,9 +46,7 @@ class TorchQwen2(torch.nn.Module):
             key = name.replace(".", "__")
             self.register_parameter(key, torch.nn.Parameter(t.to(device)))
             self.names.append(name)
-        d = cfg.head_dim
-        self.register_buffer("inv_freq", (1.0 / (cfg.rope_theta ** (torch.arange(0, d, 2, dtype=torch.int64).float()
-                                                                     / d))).to(device), persistent=False)
+        self.register_buffer("inv_freq", rope_inv_freq(cfg).to(device), persistent=False)
         self.layout = ArenaLayout.build(cfg)
 
     def p(self, name: str) -> torch.Tensor:

@@ -1,4 +1,4 @@
-"""Qwen2 / Qwen3 (dense) model description and the flat parameter arena shared by learner and sampler.
+"""Qwen2 / Qwen3 (dense) / Llama 3 model description and the flat parameter arena shared by learner and sampler.
 
 One contiguous bf16 buffer holds every parameter in the FUSED layout the token-step kernels read
 (qkv_proj = [q; k; v] rows, gate_up_proj = [gate; up] rows).  HF parameter names
@@ -10,9 +10,25 @@ per-tensor loop, no name mapping at push time.
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass, field
 
 import torch
+
+
+@dataclass(frozen=True)
+class Llama3RopeScaling:
+    """`rope_type: "llama3"` frequency scaling (Llama 3.1 / 3.2 `rope_scaling`): wavelengths above
+    original_max_position_embeddings / low_freq_factor are divided by `factor`, those below
+    original_max_position_embeddings / high_freq_factor are kept, and the band between is interpolated."""
+    factor: float
+    low_freq_factor: float
+    high_freq_factor: float
+    original_max_position_embeddings: int
+
+    def hf_dict(self) -> dict:
+        return {"factor": self.factor, "low_freq_factor": self.low_freq_factor, "high_freq_factor": self.high_freq_factor,
+                "original_max_position_embeddings": self.original_max_position_embeddings, "rope_type": "llama3"}
 
 
 @dataclass(frozen=True)
@@ -30,6 +46,8 @@ class ModelConfig:
     qk_norm: bool = False    # Qwen3: per-head RMSNorm of q and k (gains q_norm / k_norm, [head_dim]) before RoPE
     fp32_head: bool = False  # keep a bf16 residual of the head (W = hi + lo): fp32-equivalent lm_head
     lm_head_rows: int | None = None  # vocabulary rows of THIS shard's lm_head (vocab-parallel head under TP)
+    family: str = "qwen"     # "qwen" (Qwen2 / Qwen3, told apart by qk_norm) or "llama": the config.json a checkpoint gets
+    rope_scaling: Llama3RopeScaling | None = None   # None: plain RoPE, inv_freq = 1 / theta^(2i / d)
 
     @property
     def q_size(self) -> int:
@@ -90,23 +108,45 @@ class ModelConfig:
         return ModelConfig(**{**base, **kw})
 
     @staticmethod
+    def llama3_1_8b(**kw) -> "ModelConfig":
+        """Llama-3.1-8B(-Instruct)'s shapes and RoPE scaling."""
+        base = dict(vocab_size=128256, hidden_size=4096, intermediate_size=14336, num_layers=32, num_q_heads=32,
+                    num_kv_heads=8, rope_theta=500_000.0, rms_eps=1e-5, qkv_bias=False, family="llama",
+                    rope_scaling=Llama3RopeScaling(8.0, 1.0, 4.0, 8192))
+        return ModelConfig(**{**base, **kw})
+
+    @staticmethod
+    def llama3_2_3b(**kw) -> "ModelConfig":
+        """Llama-3.2-3B(-Instruct)'s shapes and RoPE scaling (its tied embeddings are stored untied here)."""
+        base = dict(vocab_size=128256, hidden_size=3072, intermediate_size=8192, num_layers=28, num_q_heads=24,
+                    num_kv_heads=8, rope_theta=500_000.0, rms_eps=1e-5, qkv_bias=False, family="llama",
+                    rope_scaling=Llama3RopeScaling(32.0, 1.0, 4.0, 8192))
+        return ModelConfig(**{**base, **kw})
+
+    @staticmethod
     def from_hf_config(d: dict) -> "ModelConfig":
-        """ModelConfig of an HF `config.json` dict of model_type "qwen2" or "qwen3" (dense).  Tied word embeddings are
-        accepted: the arena keeps an untied copy of the head (ParamArena.load_hf_state_dict)."""
+        """ModelConfig of an HF `config.json` dict of model_type "qwen2", "qwen3" (dense) or "llama" (Llama 3).  Tied
+        word embeddings are accepted: the arena keeps an untied copy of the head (ParamArena.load_hf_state_dict)."""
         mt = d.get("model_type")
-        if mt not in ("qwen2", "qwen3"):
-            raise ValueError(f"unsupported model_type {mt!r}: only 'qwen2' and 'qwen3' (dense) are implemented")
+        if mt not in ("qwen2", "qwen3", "llama"):
+            raise ValueError(f"unsupported model_type {mt!r}: only 'qwen2', 'qwen3' (dense) and 'llama' are implemented")
+        arch = {"qwen2": "Qwen2ForCausalLM", "qwen3": "Qwen3ForCausalLM", "llama": "LlamaForCausalLM"}[mt]
+        if d.get("architectures") and arch not in d["architectures"]:
+            raise ValueError(f"model_type {mt!r} does not match architectures {d['architectures']}")
         heads = int(d["num_attention_heads"])
         head_dim = int(d.get("head_dim") or d["hidden_size"] // heads)
         if head_dim != 128:
             raise ValueError(f"head_dim {head_dim} is not supported: the attention and RoPE kernels are built for 128")
         rope = d.get("rope_parameters") or {}
+        common = dict(vocab_size=int(d["vocab_size"]), hidden_size=int(d["hidden_size"]),
+                      intermediate_size=int(d["intermediate_size"]), num_layers=int(d["num_hidden_layers"]),
+                      num_q_heads=heads, num_kv_heads=int(d.get("num_key_value_heads", heads)), head_dim=head_dim,
+                      rms_eps=float(d.get("rms_norm_eps", 1e-6)))
+        if mt == "llama":
+            return ModelConfig(**common, **_llama_fields(d))
         theta = d.get("rope_theta", rope.get("rope_theta", 1_000_000.0))
-        return ModelConfig(vocab_size=int(d["vocab_size"]), hidden_size=int(d["hidden_size"]),
-                           intermediate_size=int(d["intermediate_size"]), num_layers=int(d["num_hidden_layers"]),
-                           num_q_heads=heads, num_kv_heads=int(d.get("num_key_value_heads", heads)), head_dim=head_dim,
-                           rope_theta=float(theta), rms_eps=float(d.get("rms_norm_eps", 1e-6)),
-                           qkv_bias=bool(d.get("attention_bias", mt == "qwen2")), qk_norm=mt == "qwen3")
+        return ModelConfig(**common, rope_theta=float(theta), qkv_bias=bool(d.get("attention_bias", mt == "qwen2")),
+                           qk_norm=mt == "qwen3")
 
     @staticmethod
     def tiny(**kw) -> "ModelConfig":
@@ -118,6 +158,44 @@ class ModelConfig:
 
     def num_params(self) -> int:
         return sum(n for _, n in ((name, _numel(shape)) for name, shape in fused_shapes(self)))
+
+
+def _llama_fields(d: dict) -> dict:
+    """The Llama-specific ModelConfig fields of a `config.json` dict: RoPE from `rope_scaling` (transformers 4.x, what
+    Hub checkpoints ship) or `rope_parameters` (5.x); no biases anywhere."""
+    for name in ("attention_bias", "mlp_bias"):
+        if d.get(name):
+            raise ValueError(f"{name}=true is not supported: the arena has no slot for Llama's o_proj / MLP biases")
+    rope = d.get("rope_scaling") or d.get("rope_parameters") or {}
+    kind = rope.get("rope_type", rope.get("type", "default"))
+    if kind == "default":
+        scaling = None
+    elif kind == "llama3":
+        scaling = Llama3RopeScaling(float(rope["factor"]), float(rope["low_freq_factor"]), float(rope["high_freq_factor"]),
+                                    int(rope["original_max_position_embeddings"]))
+    else:
+        raise ValueError(f"rope_type {kind!r} is not supported: only 'default' and 'llama3' are implemented")
+    theta = d.get("rope_theta", rope.get("rope_theta", 10_000.0))
+    return dict(rope_theta=float(theta), qkv_bias=False, family="llama", rope_scaling=scaling)
+
+
+def rope_inv_freq(cfg: ModelConfig) -> torch.Tensor:
+    """fp32 [head_dim / 2] RoPE inverse frequencies, the table every RoPE kernel reads.  Without scaling it is HF's
+    1 / theta^(2i / d); with Llama 3 scaling it restates transformers' `_compute_llama3_parameters` operation for
+    operation, so both tables match transformers bit for bit."""
+    d = cfg.head_dim
+    inv = 1.0 / (cfg.rope_theta ** (torch.arange(0, d, 2, dtype=torch.int64).float() / d))
+    s = cfg.rope_scaling
+    if s is None:
+        return inv
+    low_wavelen = s.original_max_position_embeddings / s.low_freq_factor
+    high_wavelen = s.original_max_position_embeddings / s.high_freq_factor
+    wavelen = 2 * math.pi / inv
+    scaled = torch.where(wavelen > low_wavelen, inv / s.factor, inv)
+    smooth = (s.original_max_position_embeddings / wavelen - s.low_freq_factor) / (s.high_freq_factor - s.low_freq_factor)
+    smoothed = (1 - smooth) * scaled / s.factor + smooth * scaled
+    medium = ~(wavelen < high_wavelen) * ~(wavelen > low_wavelen)
+    return torch.where(medium, smoothed, scaled)
 
 
 def _numel(shape) -> int:
@@ -226,7 +304,7 @@ class ParamArena:
         return self.data.numel() * self.data.element_size()
 
     def init_random(self, seed: int = 42, std: float = 0.02) -> "ParamArena":
-        """normal(0, 0.02) weights, unit norm gains (q_norm / k_norm included), zero biases — HF's Qwen2 / Qwen3
+        """normal(0, 0.02) weights, unit norm gains (q_norm / k_norm included), zero biases — HF's Qwen2 / Qwen3 / Llama
         initialisation; seed = conf/base.yaml:7."""
         g = torch.Generator(device=self.data.device).manual_seed(seed)
         for name in self.names():

@@ -28,13 +28,20 @@ def resolve(base_url: str) -> "EngineServer":
 
 
 def sampling_features(base_url: str) -> frozenset:
-    """Truncation features ("top_k", "top_p") the engine registered at `base_url` implements; empty when nothing is
-    registered there or its engine does not list any, so clients refuse such requests instead of ignoring them."""
+    """Sampling features the engine registered at `base_url` implements: the truncation it lists ("top_k", "top_p") and
+    "stop_token_ids" when it has stop sets; empty when nothing is registered there or its engine does not list any, so
+    clients refuse such requests instead of ignoring them."""
     try:
         server = resolve(base_url)
     except (ValueError, KeyError):
         return frozenset()
-    return frozenset(getattr(getattr(server, "engine", None), "sampling_features", frozenset()))
+    return engine_features(getattr(server, "engine", None))
+
+
+def engine_features(engine) -> frozenset:
+    """An engine's `sampling_features`, plus "stop_token_ids" when it sets `supports_stop_token_ids`."""
+    stop = {"stop_token_ids"} if getattr(engine, "supports_stop_token_ids", False) else set()
+    return frozenset(getattr(engine, "sampling_features", frozenset())) | stop
 
 
 @dataclass

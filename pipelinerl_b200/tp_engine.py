@@ -36,6 +36,8 @@ class TPDecodeEngine(DecodeEngine):
         if full_cfg.qk_norm:
             raise NotImplementedError("TPDecodeEngine does not implement Qwen3's q/k norm yet (qk_norm=True): "
                                       "use DecodeEngine")
+        if full_cfg.rope_scaling is not None:
+            raise NotImplementedError("TPDecodeEngine does not implement RoPE scaling yet (Llama 3): use DecodeEngine")
         if tp_size < 2 or tp_size > 8:
             raise ValueError("TPDecodeEngine is for 2..8 ranks; use DecodeEngine for tp=1")
         self.full_cfg, self.tp_rank, self.tp, self.dist, self.group = full_cfg, tp_rank, tp_size, dist, group
@@ -176,7 +178,7 @@ class TPDecodeEngine(DecodeEngine):
         _lib.check(lib.prl_sample_finalize(self._samp_buf.ptr, B, self.tp, self.sampled.data_ptr(),
                                            self.sampled_lp.data_ptr(), st))
         self._state.ignore_eos = int(self.ignore_eos)
-        _lib.check(lib.prl_advance_state(C.byref(self._state), st))
+        self._advance(st)
         _lib.check(lib.prl_tp_epoch(self.tp_epoch.data_ptr(), st))
 
     def close(self) -> None:
