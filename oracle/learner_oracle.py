@@ -1,4 +1,5 @@
-"""Oracle for hot path (2), model part: forward of the Qwen2 transformer over one PACKED row, differentiable.
+"""Oracle for hot path (2), model part: forward of the Qwen2 / Qwen3 / Llama 3 transformer over one PACKED row,
+differentiable.
 
 TEST INFRASTRUCTURE (see oracle/__init__.py).  Torch fp32 on CPU (or wherever the weights live), autograd for
 the backward.
@@ -10,14 +11,17 @@ block-diagonal causal attention for packed `position_ids` (finetune/data.py:215-
 published Qwen2 architecture, on the FUSED parameter names of pipelinerl_b200.model.fused_shapes:
 
     h = embed[ids]
-    per layer:  x = RMSNorm(h) ; qkv = x Wqkv^T + b ; q, k = RoPE(q, k; position_ids) ;
+    per layer:  x = RMSNorm(h) ; qkv = x Wqkv^T + b ; q, k = RMSNorm per head (Qwen3 only: cfg.qk_norm) ;
+                q, k = RoPE(q, k; position_ids; pipelinerl_b200.model.rope_inv_freq, llama3-scaled for Llama 3) ;
                 a = softmax(q k^T / sqrt(d) restricted to same-sample, causal) v   (GQA: q head j uses kv head j // R)
                 h = h + a Wo^T ; x = RMSNorm(h) ; h = h + (SiLU(x Wg^T) * (x Wu^T)) Wd^T
     logits = RMSNorm(h) Whead^T
 
-PINNED: tests/test_oracle_golden.py::test_learner_oracle_vs_reference_rl_step_on_hf checks this module chained with
+PINNED: tests/conformance.py::learner_oracle_vs_reference (run by tests/test_oracle_golden.py, tests/test_qwen3.py and
+tests/test_llama.py) checks this module chained with
 oracle/pg_oracle.py against tests/golden/learner_step_*.npz — the reference's own rl_step executed on HF
-Qwen2ForCausalLM (fp32, CPU): loss, the statistics and the gradient of every parameter (make_golden_learner.py).
+Qwen2ForCausalLM, Qwen3ForCausalLM and LlamaForCausalLM (fp32, CPU) for all six cases of tests/model_cases.py:
+loss, the statistics and the gradient of every parameter (make_golden_learner.py, make_golden_learner_qwen3_llama.py).
 """
 from __future__ import annotations
 
@@ -42,10 +46,11 @@ def rope(x: torch.Tensor, pos: torch.Tensor, inv_freq: torch.Tensor) -> torch.Te
 def packed_logits(cfg, w: dict[str, torch.Tensor], input_ids: torch.Tensor, position_ids: torch.Tensor) -> torch.Tensor:
     """input_ids, position_ids: [T] (positions restart at 0 for every packed sample) -> fp32 logits [T, V].
     `w` maps fused names to fp32 tensors (leaf tensors with requires_grad=True give parameter gradients)."""
+    from pipelinerl_b200.model import rope_inv_freq
     T = input_ids.numel()
     d, R = cfg.head_dim, cfg.num_q_heads // cfg.num_kv_heads
     dev = input_ids.device
-    inv_freq = 1.0 / (cfg.rope_theta ** (torch.arange(0, d, 2, dtype=torch.int64).float() / d)).to(dev)
+    inv_freq = rope_inv_freq(cfg).to(dev)
     seg = (position_ids == 0).cumsum(0)
     t = torch.arange(T, device=dev)
     allowed = (seg[:, None] == seg[None, :]) & (t[:, None] >= t[None, :])
@@ -56,9 +61,13 @@ def packed_logits(cfg, w: dict[str, torch.Tensor], input_ids: torch.Tensor, posi
         qkv = x @ w[p + "qkv_proj.weight"].t()
         if cfg.qkv_bias:
             qkv = qkv + w[p + "qkv_proj.bias"]
-        q = rope(qkv[:, :cfg.q_size].reshape(T, cfg.num_q_heads, d), position_ids, inv_freq)
-        k = rope(qkv[:, cfg.q_size:cfg.q_size + cfg.kv_size].reshape(T, cfg.num_kv_heads, d), position_ids, inv_freq)
+        q = qkv[:, :cfg.q_size].reshape(T, cfg.num_q_heads, d)
+        k = qkv[:, cfg.q_size:cfg.q_size + cfg.kv_size].reshape(T, cfg.num_kv_heads, d)
         v = qkv[:, cfg.q_size + cfg.kv_size:].reshape(T, cfg.num_kv_heads, d)
+        if cfg.qk_norm:
+            q = rmsnorm(q, w[p + "q_norm.weight"], cfg.rms_eps)
+            k = rmsnorm(k, w[p + "k_norm.weight"], cfg.rms_eps)
+        q, k = rope(q, position_ids, inv_freq), rope(k, position_ids, inv_freq)
         k, v = k.repeat_interleave(R, dim=1), v.repeat_interleave(R, dim=1)
         s = torch.einsum("thd,shd->hts", q, k) / math.sqrt(d)
         s = s.masked_fill(~allowed[None], float("-inf"))

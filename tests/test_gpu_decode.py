@@ -14,53 +14,22 @@ import pytest
 import torch
 
 from oracle.decode_oracle import OracleQwen2
+from tests import conformance
+from tests.conformance import make_engine
 from tests.helpers import GOLDEN, tiny_cfg, tiny_weights
+from tests.model_cases import CASES
 
 pytestmark = pytest.mark.gpu
 
-
-# end-to-end bounds = 1.5 x the measured differences (printed by the tests); measured on an H100:
-# max / mean |dlogprob| vs the oracle: gqa2 0.0129 / 0.0029, gqa7 0.0179 / 0.0046 (vs HF fp32: 0.0111 / 0.0030, 0.0153 / 0.0047)
-E2E_BOUNDS = {"gqa2": (1.95e-2, 4.5e-3), "gqa7": (2.7e-2, 7.1e-3)}
-
-
-def make_engine(cfg, weights, dev, **kw):
-    from pipelinerl_b200.engine import DecodeEngine
-    from pipelinerl_b200.model import ParamArena
-    arena = ParamArena(cfg, dev)
-    for name in arena.names():
-        arena.view(name).copy_(weights[name].to(torch.bfloat16))
-    return DecodeEngine(cfg, arena, device=dev, **kw)
+# Qwen2 end-to-end bounds (CASES[...]["engine"]) = 1.5 x the measured differences (printed by the tests); measured on an
+# H100: max / mean |dlogprob| vs the oracle: gqa2 0.0129 / 0.0029, gqa7 0.0179 / 0.0046 (vs HF fp32: 0.0111 / 0.0030,
+# 0.0153 / 0.0047).
 
 
 @pytest.mark.parametrize("kind", ["gqa2", "gqa7"])
 def test_teacher_forced_logprobs_match_oracle_and_hf(cuda_device, kind):
-    """Feed a 150-token sequence as the prompt (prefill-by-decode), read the logits of every step."""
-    cfg = tiny_cfg(kind)
-    w = tiny_weights(cfg)
-    eng = make_engine(cfg, w, cuda_device, max_batch=4, max_seq_len=256, max_new_tokens=8, use_cuda_graph=False,
-                      prefill_chunk=0, fused_head=False)  # prefill-by-decode; materialised logits are inspected below
-    gold = np.load(GOLDEN / f"qwen2_tiny_{kind}_T0.7.npz")
-    tokens = gold["tokens"].tolist()
-    from pipelinerl_b200.engine import SamplingParams
-    eng.temperature, eng.greedy = 0.7, True
-    eng.add_request(tokens, SamplingParams(max_tokens=2, temperature=0.7, greedy=True), model_version=0)
-    # a second, shorter sequence in another slot exercises per-slot positions / block tables
-    eng.add_request(tokens[:37], SamplingParams(max_tokens=2, temperature=0.7, greedy=True))
-    got = []
-    for t in range(len(tokens) - 1):
-        eng.step()
-        got.append(torch.log_softmax(eng.logits[0] / 0.7, -1)[tokens[t + 1]].item())
-    got = np.array(got)
-    orc = OracleQwen2(cfg, w)
-    want = orc.score(tokens, 0.7).numpy()
-    err = np.abs(got - want)
-    err_hf = np.abs(got - gold["logprobs"])
-    print(f"[decode e2e {kind}] vs oracle max {err.max():.4f} mean {err.mean():.5f} | vs HF fp32 max {err_hf.max():.4f} "
-          f"mean {err_hf.mean():.5f}  (|logprob| ~ {np.abs(want).mean():.2f})")
-    bmax, bmean = E2E_BOUNDS[kind]
-    assert err.max() <= bmax and err.mean() <= bmean, (err.max(), err.mean(), int(err.argmax()))
-    assert err_hf.max() <= bmax and err_hf.mean() <= bmean, (err_hf.max(), err_hf.mean())
+    """Feed a 150-token sequence as the prompt (prefill-by-decode), read the logits of every step (tests/conformance.py)."""
+    conformance.engine_teacher_forced(cuda_device, f"qwen2_{kind}")
 
 
 @pytest.mark.parametrize("kind,use_graph,fused", [("gqa2", True, True), ("gqa7", False, True), ("gqa2", True, False)])
@@ -85,7 +54,7 @@ def test_greedy_generation_matches_oracle(cuda_device, kind, use_graph, fused):
             top2 = torch.topk(logits, 2).values
             if float(top2[0] - top2[1]) > 5e-2:
                 assert int(torch.argmax(logits)) == tok
-            assert abs(lp - float(ref_lp[tok])) <= E2E_BOUNDS[kind][0]
+            assert abs(lp - float(ref_lp[tok])) <= CASES[f"qwen2_{kind}"]["engine"][0]
             logits = orc.forward(torch.tensor([tok]))[-1]
 
 
@@ -282,20 +251,7 @@ def test_kv_reuse_across_turns(cuda_device):
 
 @pytest.mark.parametrize("kind", ["gqa2", "gqa7"])
 def test_score_reference_logprobs(cuda_device, kind):
-    """engine.score() (chunked prefill + fused head with targets) == oracle / HF teacher-forced logprobs."""
-    cfg = tiny_cfg(kind)
-    w = tiny_weights(cfg)
-    eng = make_engine(cfg, w, cuda_device, max_batch=4, max_seq_len=256, max_new_tokens=8, prefill_chunk=64)
-    gold = np.load(GOLDEN / f"qwen2_tiny_{kind}_T0.7.npz")
-    tokens = gold["tokens"].tolist()
-    got = np.array(eng.score([tokens, tokens[:3], [5]], temperature=0.7)[0])
-    orc = OracleQwen2(cfg, w)
-    want = orc.score(tokens, 0.7).numpy()
-    assert got.shape == want.shape
-    err = np.abs(got - want)
-    assert err.max() <= 3e-2 and err.mean() <= 6e-3, (err.max(), err.mean())
-    assert np.abs(got - gold["logprobs"]).max() <= 3e-2
-    assert len(eng.free_pages) == eng.n_pages - 1 and len(eng.free_slots) == eng.B
+    conformance.engine_score(cuda_device, f"qwen2_{kind}")
 
 
 def test_per_request_sampling_parameters_share_one_batch(cuda_device):

@@ -1,24 +1,20 @@
 """Llama 3 and stop-token sets on the GPU: the state advance on scripted ids against the host stop rule (and through it
-vLLM's), the decode engine and the native learner against HF Llama fixtures, and a greedy continuation cut at a stop id
-inside the captured step.
+vLLM's), a greedy continuation cut at a stop id inside the captured step, and the decode engine and native learner
+against HF Llama fixtures (the checks of tests/conformance.py on the Llama cases).
 
-Bars: the state advance exactly; the engine at the end-to-end bar of the token-step tests (max |d logprob| <= 3e-2,
-mean <= 6e-3, greedy ids equal wherever the top-2 margin exceeds 5e-2); the learner at the bar of the Qwen2
-learner-vs-reference test (loss 2e-2 relative, every gradient 3e-2)."""
+Bars: the state advance exactly; the engine and the learner at the bounds of their case in tests/model_cases.py."""
 import ctypes as C
-import json
 
 import numpy as np
 import pytest
 import torch
 
-from tests.helpers import GOLDEN
-from tests.llama_oracle import LLAMA_KINDS, OracleLlama, llama_tiny_cfg, llama_tiny_weights
+from tests import conformance
+from tests.conformance import check_greedy, make_engine
+from tests.model_cases import CASES
 from tests.stop_rule_oracle import host_stop_rule, slot_setup, stop_cases
 
 pytestmark = pytest.mark.gpu
-
-E2E_MAX, E2E_MEAN, MARGIN = 3e-2, 6e-3, 5e-2
 
 
 # ---- state advance on scripted ids -----------------------------------------------------------------------------------
@@ -131,99 +127,7 @@ def test_advance_state_refuses_stop_ids_without_counts(cuda_device):
         _lib.check(lib.prl_advance_state(C.byref(st), None))
 
 
-# ---- decode engine vs HF ---------------------------------------------------------------------------------------------
-def _engine(cfg, w, dev, **kw):
-    from pipelinerl_b200.engine import DecodeEngine
-    from pipelinerl_b200.model import ParamArena
-    arena = ParamArena(cfg, dev)
-    for name in arena.names():
-        arena.view(name).copy_(w[name].to(torch.bfloat16))
-    return DecodeEngine(cfg, arena, device=dev, **kw)
-
-
-def _check_greedy(gold, outs, idx):
-    errs = []
-    for i, r in zip(idx, outs):
-        n = len(r.output_ids)
-        ids, lps, mg = gold["greedy_ids"][i][:n], gold["greedy_logprobs"][i][:n], gold["greedy_margin"][i][:n]
-        for t in range(n):
-            if mg[t] > MARGIN:
-                assert r.output_ids[t] == int(ids[t]), (i, t)
-            if r.output_ids[:t + 1] != ids[:t + 1].tolist():
-                break                      # a near-tie went the other way: the rest is another continuation
-            errs.append(abs(r.output_logprobs[t] - float(lps[t])))
-    assert max(errs) <= E2E_MAX and np.mean(errs) <= E2E_MEAN, (max(errs), np.mean(errs))
-    return max(errs), float(np.mean(errs))
-
-
-@pytest.mark.parametrize("kind", LLAMA_KINDS)
-def test_engine_teacher_forced_decode_path_vs_hf(cuda_device, kind):
-    from pipelinerl_b200.engine import SamplingParams
-    cfg = llama_tiny_cfg(kind)
-    w = llama_tiny_weights(cfg, kind)
-    gold = np.load(GOLDEN / f"llama_tiny_{kind}.npz")
-    tokens = gold["tokens"].tolist()
-    eng = _engine(cfg, w, cuda_device, max_batch=4, max_seq_len=384, max_new_tokens=8, use_cuda_graph=False,
-                  prefill_chunk=0)
-    eng.add_request(tokens, SamplingParams(max_tokens=2, greedy=True))
-    eng.add_request(tokens[:37], SamplingParams(max_tokens=2, greedy=True))
-    got = []
-    for t in range(len(tokens) - 1):
-        eng.step()
-        got.append(torch.log_softmax(eng.logits[0] / 0.7, -1)[tokens[t + 1]].item())
-    got = np.array(got)
-    want = OracleLlama(cfg, w).score(tokens, 0.7).numpy()
-    for ref in (gold["logprobs"], want):
-        err = np.abs(got - ref)
-        assert err.max() <= E2E_MAX and err.mean() <= E2E_MEAN, (err.max(), err.mean())
-
-
-@pytest.mark.parametrize("kind,use_graph,prefill_chunk", [("scaled", True, 1024), ("scaled", False, 0),
-                                                          ("tied", False, 1024), ("tied", True, 0), ("tied", True, 48)])
-def test_engine_greedy_vs_hf(cuda_device, kind, use_graph, prefill_chunk):
-    from pipelinerl_b200.engine import SamplingParams
-    cfg = llama_tiny_cfg(kind)
-    w = llama_tiny_weights(cfg, kind)
-    gold = np.load(GOLDEN / f"llama_tiny_{kind}.npz")
-    eng = _engine(cfg, w, cuda_device, max_batch=8, max_seq_len=320, max_new_tokens=32, use_cuda_graph=use_graph,
-                  prefill_chunk=prefill_chunk)
-    prompts = [gold["prompts"][i, :n].tolist() for i, n in enumerate(gold["prompt_len"])]
-    outs = eng.generate(prompts, SamplingParams(max_tokens=24, greedy=True))
-    print(f"[llama engine greedy {kind} graph={use_graph} chunk={prefill_chunk}]", _check_greedy(gold, outs, range(4)))
-
-
-def test_engine_prefix_sharing_matches_unshared(cuda_device):
-    from pipelinerl_b200.engine import SamplingParams
-    cfg = llama_tiny_cfg("scaled")
-    w = llama_tiny_weights(cfg, "scaled")
-    gold = np.load(GOLDEN / "llama_tiny_scaled.npz")
-    prompt = gold["prompts"][2, :gold["prompt_len"][2]].tolist()      # 230 tokens: three full shared pages
-    outs = {}
-    for share in (True, False):
-        eng = _engine(cfg, w, cuda_device, max_batch=8, max_seq_len=320, max_new_tokens=24, prefill_chunk=64,
-                      prefix_sharing=share)
-        res = eng.generate([prompt] * 6, SamplingParams(max_tokens=24, greedy=True))
-        outs[share] = [(r.output_ids, r.output_logprobs) for r in res]
-        assert (eng.stats["prefix_hits"] == 5) == share
-    for (ia, la), (ib, lb) in zip(outs[True], outs[False]):
-        assert ia == ib and np.allclose(la, lb, atol=1e-5)
-    _check_greedy(gold, [type("R", (), {"output_ids": i, "output_logprobs": l}) for i, l in outs[True]], [2] * 6)
-
-
-@pytest.mark.parametrize("kind", LLAMA_KINDS)
-def test_engine_score_vs_hf(cuda_device, kind):
-    cfg = llama_tiny_cfg(kind)
-    w = llama_tiny_weights(cfg, kind)
-    gold = np.load(GOLDEN / f"llama_tiny_{kind}.npz")
-    tokens = gold["tokens"].tolist()
-    eng = _engine(cfg, w, cuda_device, max_batch=4, max_seq_len=384, max_new_tokens=8, prefill_chunk=64)
-    got = np.array(eng.score([tokens, tokens[:3]], temperature=0.7)[0])
-    want = OracleLlama(cfg, w).score(tokens, 0.7).numpy()
-    for ref in (gold["logprobs"], want):
-        err = np.abs(got - ref)
-        assert err.max() <= E2E_MAX and err.mean() <= E2E_MEAN, (err.max(), err.mean())
-
-
+# ---- stop ids inside the captured step -------------------------------------------------------------------------------
 def _first_new(ids, at_least=1):
     """(index k, id) of the first step >= at_least whose id does not occur earlier in `ids`"""
     for k in range(at_least, len(ids)):
@@ -247,15 +151,16 @@ def test_greedy_continuation_cut_at_stop_id_inside_the_graph(cuda_device, prefil
     engine's ids dropped), and another prompt under the engine's ids.  Each output is the stop-free run's output cut at
     its first stop id, bit for bit; the others run on unchanged."""
     from pipelinerl_b200.engine import SamplingParams
-    cfg = llama_tiny_cfg("scaled")
-    w = llama_tiny_weights(cfg, "scaled")
-    gold = np.load(GOLDEN / "llama_tiny_scaled.npz")
+    case = CASES["llama_scaled"]
+    cfg = case["cfg"]
+    w = case["weights"](cfg)
+    gold = np.load(case["decode"][0])
     prompts = [gold["prompts"][i, :gold["prompt_len"][i]].tolist() for i in (0, 1, 1, 3)]
     greedy = dict(max_tokens=24, greedy=True)
     ignore = (True, False, True, False)
 
     def run(stop_ids, own):
-        eng = _engine(cfg, w, cuda_device, max_batch=8, max_seq_len=320, max_new_tokens=32, use_cuda_graph=True,
+        eng = make_engine(cfg, w, cuda_device, max_batch=8, max_seq_len=320, max_new_tokens=32, use_cuda_graph=True,
                       prefill_chunk=prefill_chunk, stop_ids=stop_ids)
         reqs = [eng.add_request(p, SamplingParams(**greedy, ignore_eos=ig, stop_token_ids=o))
                 for p, o, ig in zip(prompts, own, ignore)]
@@ -269,7 +174,7 @@ def test_greedy_continuation_cut_at_stop_id_inside_the_graph(cuda_device, prefil
         return [done[r.req_id] for r in reqs]
     free = run((), [()] * 4)
     assert all((r.finish_reason, r.stop_reason, len(r.output_ids)) == ("length", None, 24) for r in free)
-    _check_greedy(gold, free, [0, 1, 1, 3])
+    check_greedy(gold, free, [0, 1, 1, 3])
     k0, id0 = _first_new(free[0].output_ids, 3)
     k1, id1 = _first_new(free[1].output_ids, 1)
     rows = [[id0, cfg.vocab_size - 1], [id1], [], [id1]]
@@ -284,39 +189,30 @@ def test_greedy_continuation_cut_at_stop_id_inside_the_graph(cuda_device, prefil
     assert len(cut[0].output_ids) == k0 + 1 and len(cut[1].output_ids) == k1 + 1 and len(cut[2].output_ids) == 24
 
 
-# ---- native learner vs the reference's rl_step on HF Llama -----------------------------------------------------------
-@pytest.mark.parametrize("kind", LLAMA_KINDS)
+# ---- decode engine and native learner vs HF Llama (tests/conformance.py) ---------------------------------------------
+KINDS = ["scaled", "tied"]
+
+
+@pytest.mark.parametrize("kind", KINDS)
+def test_engine_teacher_forced_decode_path_vs_hf(cuda_device, kind):
+    conformance.engine_teacher_forced(cuda_device, f"llama_{kind}")
+
+
+@pytest.mark.parametrize("kind,use_graph,prefill_chunk", [("scaled", True, 1024), ("scaled", False, 0),
+                                                          ("tied", False, 1024), ("tied", True, 0), ("tied", True, 48)])
+def test_engine_greedy_vs_hf(cuda_device, kind, use_graph, prefill_chunk):
+    conformance.engine_greedy_vs_hf(cuda_device, f"llama_{kind}", use_graph, prefill_chunk)
+
+
+def test_engine_prefix_sharing_matches_unshared(cuda_device):
+    conformance.engine_prefix_sharing(cuda_device, "llama_scaled", max_seq_len=320)
+
+
+@pytest.mark.parametrize("kind", KINDS)
+def test_engine_score_vs_hf(cuda_device, kind):
+    conformance.engine_score(cuda_device, f"llama_{kind}")
+
+
+@pytest.mark.parametrize("kind", KINDS)
 def test_native_learner_vs_reference_rl_step_on_hf_llama(cuda_device, kind):
-    from pipelinerl_b200.finetune.optim import FusedAdamW
-    from pipelinerl_b200.finetune.rl import RLConfig, rl_step
-    from pipelinerl_b200.learner_model import NativeQwen2
-    from tests.helpers import batch_from_arrays
-    arrs = dict(np.load(GOLDEN / f"learner_step_llama_{kind}.npz"))
-    meta = json.loads((GOLDEN / f"learner_step_llama_{kind}.json").read_text())
-    cfg = llama_tiny_cfg(kind)
-    model = NativeQwen2(cfg, cuda_device, init=llama_tiny_weights(cfg, kind))
-    opt = FusedAdamW(model.named_parameters(), lr=1e-3, grad_dtype=torch.float32)
-    model.bind(opt)
-    for keep in (cfg.num_layers, 0):     # attention half kept by the forward / recomputed in the backward
-        model.body.keep_attention_layers = keep
-        for g in opt.grad_views().values():
-            g.zero_()
-        batch = batch_from_arrays(arrs, cuda_device)
-        loss, stats = rl_step(model, batch, meta["current_step"], meta["max_step"], RLConfig(**meta["config"]))
-        loss.backward()
-        want_loss = float(arrs["loss"])
-        loss_rel = abs(loss.item() - want_loss) / max(1.0, abs(want_loss))
-        assert loss_rel <= 2e-2, (loss.item(), want_loss)
-        worst = 0.0
-        for name, g in opt.grad_views().items():
-            key = name.replace(".", "__")
-            flat = g.reshape(-1).double().cpu()
-            want_norm = float(arrs["gnorm__" + key])
-            rel_norm = abs(float(flat.norm()) - want_norm) / (want_norm + 1e-12)
-            idx = np.unique(np.linspace(0, flat.numel() - 1, num=min(257, flat.numel())).astype(np.int64))
-            got, want = flat[torch.from_numpy(idx)].numpy(), arrs["gsamp__" + key]
-            rel = np.linalg.norm(got - want) / (np.linalg.norm(want) + 1e-12)
-            worst = max(worst, rel_norm, rel)
-            assert rel_norm <= 3e-2 and rel <= 3e-2, (name, rel_norm, rel)
-        print(f"[native learner vs reference rl_step on HF Llama, {kind}, keep={keep}] loss rel {loss_rel:.2e} "
-              f"worst gradient rel {worst:.4f}")
+    conformance.native_learner_vs_reference(cuda_device, f"llama_{kind}")

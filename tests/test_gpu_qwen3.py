@@ -1,21 +1,16 @@
-"""Qwen3 on the GPU: the q/k-norm epilogue of the token step, the learner's q/k-norm kernels, the decode engine and the
-native learner against HF Qwen3 fixtures, and the weight push.
+"""Qwen3 on the GPU: the q/k-norm epilogue of the token step, the learner's q/k-norm kernels, the weight push, and the
+decode engine and native learner against HF Qwen3 fixtures (the checks of tests/conformance.py on the Qwen3 cases).
 
-Bars: kernels against fp64 within one bf16 rounding of the output; the engine at the end-to-end bar of the Qwen2
-token-step tests (max |d logprob| <= 3e-2, mean <= 6e-3, greedy ids equal wherever the top-2 margin exceeds 5e-2); the
-learner at the bar of the Qwen2 learner-vs-reference test (loss 2e-2 relative, every gradient 3e-2)."""
-import json
-
-import numpy as np
+Bars: kernels against fp64 within one bf16 rounding of the output; the engine and the learner at the bounds of their
+case in tests/model_cases.py."""
 import pytest
 import torch
 
-from tests.helpers import GOLDEN
-from tests.qwen3_oracle import QWEN3_KINDS, OracleQwen3, qwen3_tiny_cfg, qwen3_tiny_weights
+from tests import conformance
+from tests.model_cases import qwen3_tiny_cfg, qwen3_tiny_weights
 
 pytestmark = pytest.mark.gpu
 
-E2E_MAX, E2E_MEAN, MARGIN = 3e-2, 6e-3, 5e-2
 D = 128
 
 
@@ -198,101 +193,7 @@ def test_learner_qk_norm_rope_fwd_bwd_vs_autograd(cuda_device, T, n_q, n_kv):
     assert torch.equal(y, y3)
 
 
-# ---- decode engine -------------------------------------------------------------------------------------------------
-def _engine(cfg, w, dev, **kw):
-    from pipelinerl_b200.engine import DecodeEngine
-    from pipelinerl_b200.model import ParamArena
-    arena = ParamArena(cfg, dev)
-    for name in arena.names():
-        arena.view(name).copy_(w[name].to(torch.bfloat16))
-    return DecodeEngine(cfg, arena, device=dev, **kw)
-
-
-def _check_greedy(gold, outs, idx):
-    errs = []
-    for i, r in zip(idx, outs):
-        n = len(r.output_ids)
-        ids, lps, mg = gold["greedy_ids"][i][:n], gold["greedy_logprobs"][i][:n], gold["greedy_margin"][i][:n]
-        for t in range(n):
-            if mg[t] > MARGIN:
-                assert r.output_ids[t] == int(ids[t]), (i, t)
-            if r.output_ids[:t + 1] != ids[:t + 1].tolist():
-                break                      # a near-tie went the other way: the rest is another continuation
-            errs.append(abs(r.output_logprobs[t] - float(lps[t])))
-    assert max(errs) <= E2E_MAX and np.mean(errs) <= E2E_MEAN, (max(errs), np.mean(errs))
-    return max(errs), float(np.mean(errs))
-
-
-@pytest.mark.parametrize("kind", QWEN3_KINDS)
-def test_engine_teacher_forced_decode_path_vs_hf(cuda_device, kind):
-    """prompt fed through the decode step (prefill_chunk=0), logits of every step vs HF fp32 and the oracle"""
-    from pipelinerl_b200.engine import SamplingParams
-    cfg = qwen3_tiny_cfg(kind)
-    w = qwen3_tiny_weights(cfg)
-    gold = np.load(GOLDEN / f"qwen3_tiny_{kind}.npz")
-    tokens = gold["tokens"].tolist()
-    eng = _engine(cfg, w, cuda_device, max_batch=4, max_seq_len=256, max_new_tokens=8, use_cuda_graph=False,
-                  prefill_chunk=0)
-    eng.add_request(tokens, SamplingParams(max_tokens=2, greedy=True))
-    eng.add_request(tokens[:37], SamplingParams(max_tokens=2, greedy=True))
-    got = []
-    for t in range(len(tokens) - 1):
-        eng.step()
-        got.append(torch.log_softmax(eng.logits[0] / 0.7, -1)[tokens[t + 1]].item())
-    got = np.array(got)
-    want = OracleQwen3(cfg, w).score(tokens, 0.7).numpy()
-    for ref in (gold["logprobs"], want):
-        err = np.abs(got - ref)
-        assert err.max() <= E2E_MAX and err.mean() <= E2E_MEAN, (err.max(), err.mean())
-    print(f"[qwen3 engine decode-path {kind}] vs HF max {np.abs(got - gold['logprobs']).max():.4f}")
-
-
-@pytest.mark.parametrize("kind,use_graph,prefill_chunk", [("wide", True, 1024), ("wide", False, 0), ("gqa4", False, 1024),
-                                                          ("gqa4", True, 0), ("gqa4", True, 48)])
-def test_engine_greedy_vs_hf(cuda_device, kind, use_graph, prefill_chunk):
-    from pipelinerl_b200.engine import SamplingParams
-    cfg = qwen3_tiny_cfg(kind)
-    w = qwen3_tiny_weights(cfg)
-    gold = np.load(GOLDEN / f"qwen3_tiny_{kind}.npz")
-    eng = _engine(cfg, w, cuda_device, max_batch=8, max_seq_len=320, max_new_tokens=32, use_cuda_graph=use_graph,
-                  prefill_chunk=prefill_chunk)
-    prompts = [gold["prompts"][i, :n].tolist() for i, n in enumerate(gold["prompt_len"])]
-    outs = eng.generate(prompts, SamplingParams(max_tokens=24, greedy=True))
-    print(f"[qwen3 engine greedy {kind} graph={use_graph} chunk={prefill_chunk}] max/mean", _check_greedy(gold, outs, range(len(prompts))))
-
-
-def test_engine_prefix_sharing_matches_unshared(cuda_device):
-    from pipelinerl_b200.engine import SamplingParams
-    cfg = qwen3_tiny_cfg("wide")
-    w = qwen3_tiny_weights(cfg)
-    gold = np.load(GOLDEN / "qwen3_tiny_wide.npz")
-    prompt = gold["prompts"][2, :gold["prompt_len"][2]].tolist()      # 130 tokens: two full shared pages
-    outs = {}
-    for share in (True, False):
-        eng = _engine(cfg, w, cuda_device, max_batch=8, max_seq_len=256, max_new_tokens=24, prefill_chunk=64,
-                      prefix_sharing=share)
-        res = eng.generate([prompt] * 6, SamplingParams(max_tokens=24, greedy=True))
-        outs[share] = [(r.output_ids, r.output_logprobs) for r in res]
-        assert (eng.stats["prefix_hits"] == 5) == share
-    for (ia, la), (ib, lb) in zip(outs[True], outs[False]):
-        assert ia == ib and np.allclose(la, lb, atol=1e-5)
-    _check_greedy(gold, [type("R", (), {"output_ids": i, "output_logprobs": l}) for i, l in outs[True]], [2] * 6)
-
-
-@pytest.mark.parametrize("kind", QWEN3_KINDS)
-def test_engine_score_vs_hf(cuda_device, kind):
-    cfg = qwen3_tiny_cfg(kind)
-    w = qwen3_tiny_weights(cfg)
-    gold = np.load(GOLDEN / f"qwen3_tiny_{kind}.npz")
-    tokens = gold["tokens"].tolist()
-    eng = _engine(cfg, w, cuda_device, max_batch=4, max_seq_len=256, max_new_tokens=8, prefill_chunk=64)
-    got = np.array(eng.score([tokens, tokens[:3]], temperature=0.7)[0])
-    want = OracleQwen3(cfg, w).score(tokens, 0.7).numpy()
-    for ref in (gold["logprobs"], want):
-        err = np.abs(got - ref)
-        assert err.max() <= E2E_MAX and err.mean() <= E2E_MEAN, (err.max(), err.mean())
-
-
+# ---- weight push ---------------------------------------------------------------------------------------------------
 def test_pushed_qwen3_arena_samples_the_same_ids(cuda_device):
     """a Qwen3 arena pushed as raw bytes into a receiver's buffer: the receiving engine samples (T = 1) the same ids
     and logprobs as an engine on the learner's arena"""
@@ -324,41 +225,30 @@ def test_pushed_qwen3_arena_samples_the_same_ids(cuda_device):
     recv.close()
 
 
-# ---- native learner vs the reference's rl_step on HF Qwen3 -----------------------------------------------------------
-@pytest.mark.parametrize("kind", QWEN3_KINDS)
+# ---- decode engine and native learner vs HF Qwen3 (tests/conformance.py) ---------------------------------------------
+KINDS = ["wide", "gqa4"]
+
+
+@pytest.mark.parametrize("kind", KINDS)
+def test_engine_teacher_forced_decode_path_vs_hf(cuda_device, kind):
+    conformance.engine_teacher_forced(cuda_device, f"qwen3_{kind}")
+
+
+@pytest.mark.parametrize("kind,use_graph,prefill_chunk", [("wide", True, 1024), ("wide", False, 0), ("gqa4", False, 1024),
+                                                          ("gqa4", True, 0), ("gqa4", True, 48)])
+def test_engine_greedy_vs_hf(cuda_device, kind, use_graph, prefill_chunk):
+    conformance.engine_greedy_vs_hf(cuda_device, f"qwen3_{kind}", use_graph, prefill_chunk)
+
+
+def test_engine_prefix_sharing_matches_unshared(cuda_device):
+    conformance.engine_prefix_sharing(cuda_device, "qwen3_wide", max_seq_len=256)
+
+
+@pytest.mark.parametrize("kind", KINDS)
+def test_engine_score_vs_hf(cuda_device, kind):
+    conformance.engine_score(cuda_device, f"qwen3_{kind}")
+
+
+@pytest.mark.parametrize("kind", KINDS)
 def test_native_learner_vs_reference_rl_step_on_hf_qwen3(cuda_device, kind):
-    from pipelinerl_b200.finetune.optim import FusedAdamW
-    from pipelinerl_b200.finetune.rl import RLConfig, rl_step
-    from pipelinerl_b200.learner_model import NativeQwen2
-    from tests.helpers import batch_from_arrays
-    arrs = dict(np.load(GOLDEN / f"learner_step_qwen3_{kind}.npz"))
-    meta = json.loads((GOLDEN / f"learner_step_qwen3_{kind}.json").read_text())
-    cfg = qwen3_tiny_cfg(kind)
-    model = NativeQwen2(cfg, cuda_device, init=qwen3_tiny_weights(cfg))
-    opt = FusedAdamW(model.named_parameters(), lr=1e-3, grad_dtype=torch.float32)
-    model.bind(opt)
-    for keep in (cfg.num_layers, 0):     # attention half kept by the forward / recomputed in the backward
-        model.body.keep_attention_layers = keep
-        for g in opt.grad_views().values():
-            g.zero_()
-        batch = batch_from_arrays(arrs, cuda_device)
-        loss, stats = rl_step(model, batch, meta["current_step"], meta["max_step"], RLConfig(**meta["config"]))
-        loss.backward()
-        want_loss = float(arrs["loss"])
-        loss_rel = abs(loss.item() - want_loss) / max(1.0, abs(want_loss))
-        assert loss_rel <= 2e-2, (loss.item(), want_loss)
-        worst = 0.0
-        grads = opt.grad_views()
-        assert {n for n in grads if "_norm" in n} >= {f"layers.{l}.{k}_norm.weight" for l in range(2) for k in "qk"}
-        for name, g in grads.items():
-            key = name.replace(".", "__")
-            flat = g.reshape(-1).double().cpu()
-            want_norm = float(arrs["gnorm__" + key])
-            rel_norm = abs(float(flat.norm()) - want_norm) / (want_norm + 1e-12)
-            idx = np.unique(np.linspace(0, flat.numel() - 1, num=min(257, flat.numel())).astype(np.int64))
-            got, want = flat[torch.from_numpy(idx)].numpy(), arrs["gsamp__" + key]
-            rel = np.linalg.norm(got - want) / (np.linalg.norm(want) + 1e-12)
-            worst = max(worst, rel_norm, rel)
-            assert rel_norm <= 3e-2 and rel <= 3e-2, (name, rel_norm, rel)
-        print(f"[native learner vs reference rl_step on HF Qwen3, {kind}, keep={keep}] loss rel {loss_rel:.2e} "
-              f"worst gradient rel {worst:.4f}")
+    conformance.native_learner_vs_reference(cuda_device, f"qwen3_{kind}")

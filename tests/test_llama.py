@@ -1,8 +1,5 @@
-"""Llama 3 support without a GPU: the RoPE table, the model description, the checkpoint format and the Llama oracle
-against HF.
-
-End-to-end bar (the one the token-step tests use): max |d logprob| <= 3e-2, mean <= 6e-3, and greedy ids equal wherever
-the top-2 logit margin exceeds 5e-2."""
+"""Llama 3 support without a GPU: the RoPE table, the model description, the checkpoint format and the oracles against
+HF Llama and the reference (the checks of tests/conformance.py on the Llama cases of tests/model_cases.py)."""
 import hashlib
 import json
 import math
@@ -11,10 +8,10 @@ import numpy as np
 import pytest
 import torch
 
-from tests.helpers import GOLDEN
-from tests.llama_oracle import LLAMA_KINDS, TIED, OracleLlama, hf_llama_model, llama_tiny_cfg, llama_tiny_weights
+from tests import conformance
+from tests.model_cases import CASES, hf_model, llama_tiny_cfg, llama_tiny_weights
 
-E2E_MAX, E2E_MEAN, MARGIN = 3e-2, 6e-3, 5e-2
+KINDS = ["scaled", "tied"]
 
 # config.json of meta-llama/Llama-3.1-8B-Instruct and meta-llama/Llama-3.2-3B as published (transformers 4.x format)
 LLAMA31_8B_INSTRUCT = {
@@ -80,52 +77,42 @@ def test_scaled_fixture_config_has_all_three_bands():
     assert ((got[mid] < base[mid]) & (got[mid] > base[mid] / s.factor)).all()
 
 
-# ---- oracle vs HF ----------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("kind", LLAMA_KINDS)
+# ---- oracles vs HF and the reference ---------------------------------------------------------------------------------
+@pytest.mark.parametrize("kind", KINDS)
 def test_llama_oracle_teacher_forced_vs_hf(kind):
-    cfg = llama_tiny_cfg(kind)
-    gold = np.load(GOLDEN / f"llama_tiny_{kind}.npz")
-    tokens = gold["tokens"].tolist()
-    w = llama_tiny_weights(cfg, kind)
-    got = OracleLlama(cfg, w).score(tokens, float(gold["temperature"])).numpy()
-    err = np.abs(got - gold["logprobs"])
-    print(f"[llama oracle vs HF {kind}] max {err.max():.4f} mean {err.mean():.5f}")
-    assert err.max() <= E2E_MAX and err.mean() <= E2E_MEAN, (err.max(), err.mean())
-    if kind == "scaled":   # the scaled table is visible in the logprobs: the unscaled one misses the bar
-        from dataclasses import replace
-
-        from oracle.decode_oracle import OracleQwen2
-        plain = OracleQwen2(replace(cfg, rope_scaling=None), w).score(tokens, float(gold["temperature"])).numpy()
-        assert np.abs(plain - gold["logprobs"]).max() > 10 * err.max()
+    conformance.decode_oracle_vs_hf(f"llama_{kind}")
 
 
-@pytest.mark.parametrize("kind", LLAMA_KINDS)
+@pytest.mark.parametrize("kind", KINDS)
 def test_llama_oracle_greedy_vs_hf(kind):
-    cfg = llama_tiny_cfg(kind)
-    gold = np.load(GOLDEN / f"llama_tiny_{kind}.npz")
-    orc = OracleLlama(cfg, llama_tiny_weights(cfg, kind))
-    errs = []
-    for i, n in enumerate(gold["prompt_len"]):
-        orc.reset()
-        logits = orc.forward(torch.tensor(gold["prompts"][i, :n]))[-1]
-        for t, tok in enumerate(gold["greedy_ids"][i].tolist()):      # replay HF's continuation through the oracle
-            if gold["greedy_margin"][i, t] > MARGIN:
-                assert int(torch.argmax(logits)) == tok, (i, t)
-            errs.append(abs(float(torch.log_softmax(logits, -1)[tok]) - float(gold["greedy_logprobs"][i, t])))
-            logits = orc.forward(torch.tensor([tok]))[-1]
-    assert max(errs) <= E2E_MAX and np.mean(errs) <= E2E_MEAN, (max(errs), np.mean(errs))
+    conformance.decode_oracle_greedy_vs_hf(f"llama_{kind}")
 
 
-@pytest.mark.parametrize("kind", LLAMA_KINDS)
+@pytest.mark.parametrize("kind", KINDS)
 def test_torch_llama_module_matches_hf_in_fp32(kind):
-    """learner_model.TorchQwen2 on a Llama config (the learner tests' fp32 second opinion) equals HF Llama in fp32."""
-    from pipelinerl_b200.learner_model import TorchQwen2
-    cfg = llama_tiny_cfg(kind)
-    gold = np.load(GOLDEN / f"llama_tiny_{kind}.npz")
-    tokens = torch.from_numpy(gold["tokens"])
-    with torch.no_grad():
-        logits = TorchQwen2(cfg, "cpu", init=llama_tiny_weights(cfg, kind))(tokens[None]).logits[0]
-    np.testing.assert_allclose(logits[-4:].numpy(), gold["last_logits"], atol=2e-4, rtol=1e-4)
+    conformance.torch_module_matches_hf(f"llama_{kind}")
+
+
+@pytest.mark.parametrize("kind", KINDS)
+def test_learner_oracle_vs_reference_rl_step_on_hf_llama(kind):
+    conformance.learner_oracle_vs_reference(f"llama_{kind}")
+
+
+# ---- oracle vs HF: the scaled table is visible in the logprobs --------------------------------------------------------
+def test_unscaled_rope_table_misses_the_hf_bar():
+    """tests/test_oracle_golden.py holds the oracle at the end-to-end bar against HF Llama; with the unscaled table it
+    misses that bar on the scaled configuration by more than 10 x."""
+    from dataclasses import replace
+
+    from oracle.decode_oracle import OracleQwen2
+    case = CASES["llama_scaled"]
+    cfg = case["cfg"]
+    w = case["weights"](cfg)
+    gold = np.load(case["decode"][0])
+    tokens, temp = gold["tokens"].tolist(), float(gold["temperature"])
+    err = np.abs(OracleQwen2(cfg, w).score(tokens, temp).numpy() - gold["logprobs"])
+    plain = OracleQwen2(replace(cfg, rope_scaling=None), w).score(tokens, temp).numpy()
+    assert np.abs(plain - gold["logprobs"]).max() > 10 * err.max()
 
 
 # ---- model description -----------------------------------------------------------------------------------------------
@@ -228,40 +215,16 @@ def test_llama_layout_is_qwen2_without_biases():
 
 
 # ---- checkpoints -----------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("kind", LLAMA_KINDS)
+@pytest.mark.parametrize("kind", KINDS)
 def test_llama_checkpoint_round_trip_and_opens_in_hf(tmp_path, kind):
-    """save_model_only -> HF AutoModelForCausalLM loads it as Llama (with its RoPE scaling) and its fp32 logits match
-    the arena's (the oracle on the same weights); load_model_weights returns every fused tensor bit for bit."""
-    from transformers import AutoModelForCausalLM
-
-    from pipelinerl_b200.finetune.checkpoints import load_model_weights, save_model_only
-    from pipelinerl_b200.model import fused_shapes
-    cfg = llama_tiny_cfg(kind)
-    w = llama_tiny_weights(cfg, kind)
-    save_model_only(tmp_path / "ckpt", cfg, [(n, w[n]) for n, _ in fused_shapes(cfg)])
-    back = load_model_weights(tmp_path / "ckpt", cfg)
-    assert set(back) == set(w)
-    for n in w:
-        assert torch.equal(back[n].float(), w[n]), n
-    hf = AutoModelForCausalLM.from_pretrained(str(tmp_path / "ckpt"), dtype=torch.float32,
-                                              attn_implementation="eager").eval()
-    assert type(hf).__name__ == "LlamaForCausalLM"
-    tokens = torch.from_numpy(np.load(GOLDEN / f"llama_tiny_{kind}.npz")["tokens"][:200])
-    with torch.no_grad():
-        got = torch.log_softmax(hf(input_ids=tokens[None]).logits[0].float(), -1)
-    want = torch.log_softmax(OracleLlama(cfg, w).forward(tokens), -1)
-    err = (got - want).abs()
-    assert err.max().item() <= E2E_MAX and err.mean().item() <= E2E_MEAN, (err.max().item(), err.mean().item())
-    with torch.no_grad():
-        direct = torch.log_softmax(hf_llama_model(cfg, w, tied=TIED[kind]).eval()(input_ids=tokens[None]).logits[0], -1)
-    assert torch.allclose(got, direct, atol=1e-5)
+    conformance.checkpoint_round_trip_opens_in_hf(tmp_path, f"llama_{kind}", n_tokens=200)
 
 
 def test_tied_checkpoint_loads_untied_into_the_arena():
     from pipelinerl_b200.model import ParamArena
     cfg = llama_tiny_cfg("tied")
-    w = llama_tiny_weights(cfg, "tied")
-    sd = hf_llama_model(cfg, w, tied=True).state_dict()
+    w = llama_tiny_weights(cfg, tied=True)
+    sd = hf_model(cfg, w, tied=True).state_dict()
     sd = {k: v for k, v in sd.items() if "rotary" not in k and k != "lm_head.weight"}
     arena = ParamArena(cfg, "cpu")
     arena.load_hf_state_dict(sd)

@@ -1,58 +1,34 @@
-"""Qwen3 support without a GPU: the model description, the checkpoint format and the Qwen3 oracle against HF.
-
-End-to-end bar (the one the token-step tests use): max |d logprob| <= 3e-2, mean <= 6e-3, and greedy ids equal wherever
-the top-2 logit margin exceeds 5e-2."""
+"""Qwen3 support without a GPU: the model description, the checkpoint format and the oracles against HF Qwen3 and the
+reference (the checks of tests/conformance.py on the Qwen3 cases of tests/model_cases.py)."""
 import hashlib
 
-import numpy as np
 import pytest
 import torch
 
-from tests.helpers import GOLDEN
-from tests.qwen3_oracle import QWEN3_KINDS, OracleQwen3, hf_qwen3_model, qwen3_tiny_cfg, qwen3_tiny_weights
+from tests import conformance
+from tests.model_cases import qwen3_tiny_cfg
 
-E2E_MAX, E2E_MEAN, MARGIN = 3e-2, 6e-3, 5e-2
+KINDS = ["wide", "gqa4"]
 
 
-@pytest.mark.parametrize("kind", QWEN3_KINDS)
+@pytest.mark.parametrize("kind", KINDS)
 def test_qwen3_oracle_teacher_forced_vs_hf(kind):
-    cfg = qwen3_tiny_cfg(kind)
-    gold = np.load(GOLDEN / f"qwen3_tiny_{kind}.npz")
-    tokens = gold["tokens"].tolist()
-    got = OracleQwen3(cfg, qwen3_tiny_weights(cfg)).score(tokens, float(gold["temperature"])).numpy()
-    err = np.abs(got - gold["logprobs"])
-    print(f"[qwen3 oracle vs HF {kind}] max {err.max():.4f} mean {err.mean():.5f}")
-    assert err.max() <= E2E_MAX and err.mean() <= E2E_MEAN, (err.max(), err.mean())
+    conformance.decode_oracle_vs_hf(f"qwen3_{kind}")
 
 
-@pytest.mark.parametrize("kind", QWEN3_KINDS)
+@pytest.mark.parametrize("kind", KINDS)
 def test_qwen3_oracle_greedy_vs_hf(kind):
-    cfg = qwen3_tiny_cfg(kind)
-    gold = np.load(GOLDEN / f"qwen3_tiny_{kind}.npz")
-    orc = OracleQwen3(cfg, qwen3_tiny_weights(cfg))
-    errs = []
-    for i, n in enumerate(gold["prompt_len"]):
-        orc.reset()
-        logits = orc.forward(torch.tensor(gold["prompts"][i, :n]))[-1]
-        for t, tok in enumerate(gold["greedy_ids"][i].tolist()):      # replay HF's continuation through the oracle
-            if gold["greedy_margin"][i, t] > MARGIN:
-                assert int(torch.argmax(logits)) == tok, (i, t)
-            errs.append(abs(float(torch.log_softmax(logits, -1)[tok]) - float(gold["greedy_logprobs"][i, t])))
-            logits = orc.forward(torch.tensor([tok]))[-1]
-    assert max(errs) <= E2E_MAX and np.mean(errs) <= E2E_MEAN, (max(errs), np.mean(errs))
+    conformance.decode_oracle_greedy_vs_hf(f"qwen3_{kind}")
 
 
-@pytest.mark.parametrize("kind", QWEN3_KINDS)
+@pytest.mark.parametrize("kind", KINDS)
 def test_torch_qwen3_module_matches_hf_in_fp32(kind):
-    """learner_model.TorchQwen2 with qk_norm (the learner tests' fp32 second opinion) equals HF Qwen3 in fp32."""
-    from pipelinerl_b200.learner_model import TorchQwen2
-    cfg = qwen3_tiny_cfg(kind)
-    w = qwen3_tiny_weights(cfg)
-    gold = np.load(GOLDEN / f"qwen3_tiny_{kind}.npz")
-    tokens = torch.from_numpy(gold["tokens"])
-    with torch.no_grad():
-        logits = TorchQwen2(cfg, "cpu", init=w)(tokens[None]).logits[0]
-    np.testing.assert_allclose(logits[-4:].numpy(), gold["last_logits"], atol=2e-4, rtol=1e-4)
+    conformance.torch_module_matches_hf(f"qwen3_{kind}")
+
+
+@pytest.mark.parametrize("kind", KINDS)
+def test_learner_oracle_vs_reference_rl_step_on_hf_qwen3(kind):
+    conformance.learner_oracle_vs_reference(f"qwen3_{kind}")
 
 
 # ---- model description ---------------------------------------------------------------------------------------------
@@ -179,32 +155,7 @@ def test_from_hf_config_reads_published_configs_and_rejects_others():
 
 # ---- checkpoints ----------------------------------------------------------------------------------------------------
 def test_qwen3_checkpoint_round_trip_and_opens_in_hf(tmp_path):
-    """save_model_only -> HF AutoModelForCausalLM loads it as Qwen3 and computes the oracle's logits; load_model_weights
-    returns every fused tensor (q/k gains included) bit for bit."""
-    from transformers import AutoModelForCausalLM
-
-    from pipelinerl_b200.finetune.checkpoints import load_model_weights, save_model_only
-    from pipelinerl_b200.model import fused_shapes
-    cfg = qwen3_tiny_cfg("wide")
-    w = qwen3_tiny_weights(cfg)
-    save_model_only(tmp_path / "ckpt", cfg, [(n, w[n]) for n, _ in fused_shapes(cfg)])
-    back = load_model_weights(tmp_path / "ckpt", cfg)
-    assert set(back) == set(w)
-    for n in w:
-        assert torch.equal(back[n].float(), w[n]), n
-    hf = AutoModelForCausalLM.from_pretrained(str(tmp_path / "ckpt"), dtype=torch.float32,
-                                              attn_implementation="eager").eval()
-    assert type(hf).__name__ == "Qwen3ForCausalLM"
-    tokens = torch.from_numpy(np.load(GOLDEN / "qwen3_tiny_wide.npz")["tokens"][:64])
-    with torch.no_grad():
-        got = torch.log_softmax(hf(input_ids=tokens[None]).logits[0].float(), -1)
-    want = torch.log_softmax(OracleQwen3(cfg, w).forward(tokens), -1)
-    err = (got - want).abs()
-    assert err.max().item() <= E2E_MAX and err.mean().item() <= E2E_MEAN, (err.max().item(), err.mean().item())
-    # and the HF model built directly from the weights agrees with the reloaded one (nothing lost on disk)
-    with torch.no_grad():
-        direct = torch.log_softmax(hf_qwen3_model(cfg, w).eval()(input_ids=tokens[None]).logits[0].float(), -1)
-    assert torch.allclose(got, direct, atol=1e-5)
+    conformance.checkpoint_round_trip_opens_in_hf(tmp_path, "qwen3_wide", n_tokens=64)
 
 
 def test_tp_engine_refuses_qk_norm():
