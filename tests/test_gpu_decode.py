@@ -87,16 +87,40 @@ def test_sampling_distribution_and_logprob_capture(cuda_device):
     assert (ids.cpu() == int(torch.argmax(logits[0].cpu()))).all()
 
 
+# (n_q, n_kv) -> context lengths.  R = n_q / n_kv query heads share a kv head and are the rows of one 16-row MMA tile:
+# 7 (Qwen2.5-7B, at BASELINE-like context), 4 (Qwen3-8B, Llama-3.1-8B), 5 (Qwen3-14B, Qwen2.5-32B), 3 (Llama-3.2-3B),
+# 6 (Qwen2.5-1.5B), 1 (MHA) and 16, the widest grouping the ABI takes, whose heads 8..15 are the tile's second row half.
+# 0 is an idle slot; 16, 63, 64 and 65 end inside, at the end of and just past the first page.
+_DECODE_GROUPINGS = {
+    (28, 4): [8192, 8191, 1, 65, 12000, 640, 0, 16, 63, 64],
+    (32, 8): [0, 16, 63, 64, 65, 2100],
+    (40, 8): [1, 16, 63, 64, 700, 0],
+    (24, 8): [64, 0, 63, 16, 1300],
+    (12, 2): [16, 63, 64, 0, 999],
+    (8, 8): [63, 64, 16, 1, 0, 1500],
+    (32, 2): [0, 16, 63, 64, 65, 3000],
+}
+
+
 def test_paged_attention_long_context_vs_fp32(cuda_device):
-    """Decode attention alone at BASELINE-like context (8192+ tokens, 7:1 GQA, ragged lengths, scattered pages)."""
+    """Decode attention alone at every GQA grouping the supported models use (ragged lengths, scattered pages), through
+    both merges of the context splits: the combine kernel, and the in-kernel merge by the last split to arrive
+    (prl_attn_set_fused_combine), which must give the same bits and re-arm its arrival tickets for the next call."""
     from pipelinerl_b200 import _lib
     lib = _lib.load()
-    dev = cuda_device
-    B, n_q, n_kv, D, P = 6, 28, 4, 128, 64
-    lens = [8192, 8191, 1, 65, 12000, 640]
+    try:
+        for (n_q, n_kv), lens in _DECODE_GROUPINGS.items():
+            _check_decode_attention(lib, cuda_device, n_q, n_kv, lens)
+    finally:
+        _lib.check(lib.prl_attn_set_fused_combine(0))
+
+
+def _check_decode_attention(lib, dev, n_q, n_kv, lens):
+    from pipelinerl_b200 import _lib
+    B, D, P = len(lens), 128, 64
     max_blocks = 192
     n_pages = 1 + sum((l + P - 1) // P for l in lens) + 5
-    g = torch.Generator().manual_seed(5)
+    g = torch.Generator().manual_seed(5 + n_q + 100 * n_kv)
     L, layer = 2, 1
     kv = (torch.randn(L * 2 * n_pages * n_kv * P * D, generator=g) * 0.5).to(torch.bfloat16).to(dev)
     kv5 = kv.view(L, 2, n_pages, n_kv, P, D)
@@ -109,23 +133,38 @@ def test_paged_attention_long_context_vs_fp32(cuda_device):
         at += k
     q = (torch.randn(B, n_q, D, generator=g)).to(torch.bfloat16).to(dev)
     bt_d, sl_d = bt.to(dev), torch.tensor(lens, dtype=torch.int32, device=dev)
-    out = torch.zeros(B, n_q * D, dtype=torch.bfloat16, device=dev)
-    for splits in (1, 4, int(lib.prl_paged_attn_splits(B, n_kv, max(lens)))):
+    refs = []
+    for b, l in enumerate(lens):
+        k = (l + P - 1) // P
+        pages = bt[b, :k].long().to(dev)
+        K = kv5[layer, 0, pages].permute(1, 0, 2, 3).reshape(n_kv, k * P, D)[:, :l].float()
+        V = kv5[layer, 1, pages].permute(1, 0, 2, 3).reshape(n_kv, k * P, D)[:, :l].float()
+        qb = q[b].float().view(n_kv, n_q // n_kv, D)
+        s = torch.einsum("grd,gsd->grs", qb, K) / D ** 0.5
+        refs.append(torch.einsum("grs,gsd->grd", torch.softmax(s, -1), V).reshape(-1))
+    worst = 0.0
+    for splits in (1, 3, 4, int(lib.prl_paged_attn_splits(B, n_kv, max(lens)))):
         ws = torch.zeros(int(lib.prl_paged_attn_workspace_bytes(B, n_q, splits)), dtype=torch.uint8, device=dev)
-        _lib.check(lib.prl_paged_attn_decode(q.data_ptr(), kv.data_ptr(), n_pages, L, layer, bt_d.data_ptr(), max_blocks,
-                                             sl_d.data_ptr(), B, n_q, n_kv, D, P, splits, 1.0 / D ** 0.5, out.data_ptr(),
-                                             ws.data_ptr(), ws.numel(), None))
-        torch.cuda.synchronize()
+        outs = []
+        for fused in (0, 1, 1):            # the second fused call runs on the tickets the first one left behind
+            _lib.check(lib.prl_attn_set_fused_combine(fused))
+            out = torch.full((B, n_q * D), 3.0, dtype=torch.bfloat16, device=dev)
+            _lib.check(lib.prl_paged_attn_decode(q.data_ptr(), kv.data_ptr(), n_pages, L, layer, bt_d.data_ptr(),
+                                                 max_blocks, sl_d.data_ptr(), B, n_q, n_kv, D, P, splits,
+                                                 1.0 / D ** 0.5, out.data_ptr(), ws.data_ptr(), ws.numel(), None))
+            torch.cuda.synchronize()
+            outs.append(out)
+        out = outs[0]
+        assert torch.equal(outs[1], out) and torch.equal(outs[2], out), (n_q, n_kv, splits)
         for b, l in enumerate(lens):
-            k = (l + P - 1) // P
-            pages = bt[b, :k].long().to(dev)
-            K = kv5[layer, 0, pages].permute(1, 0, 2, 3).reshape(n_kv, k * P, D)[:, :l].float()
-            V = kv5[layer, 1, pages].permute(1, 0, 2, 3).reshape(n_kv, k * P, D)[:, :l].float()
-            qb = q[b].float().view(n_kv, n_q // n_kv, D)
-            s = torch.einsum("grd,gsd->grs", qb, K) / D ** 0.5
-            ref = torch.einsum("grs,gsd->grd", torch.softmax(s, -1), V).reshape(-1)
+            if l == 0:                     # idle slot: nothing to attend to, the output row is zero
+                assert (out[b] == 0).all(), (n_q, n_kv, splits)
+                continue
+            ref = refs[b]
             err = (out[b].float() - ref).abs().max().item()
-            assert err <= 4e-3 * max(1.0, ref.abs().max().item()), (splits, b, err)
+            worst = max(worst, err / max(1.0, ref.abs().max().item()))
+            assert err <= 4e-3 * max(1.0, ref.abs().max().item()), (n_q, n_kv, splits, b, err)
+    print(f"[decode attention {n_q}/{n_kv}] max |err| / max(1, |ref|) {worst:.2e} over lengths {lens}")
 
 
 def test_prefix_sharing_and_chunked_prefill(cuda_device):
@@ -171,6 +210,10 @@ def test_prefix_sharing_and_chunked_prefill(cuda_device):
     (4, 2, [(0, 300), (129, 70), (64, 1)]),        # R = 2; chunk starting mid-page; single-row chunk
     (8, 8, [(500, 129), (0, 128)]),                # R = 1 (MHA): 128 tokens per tile
     (8, 1, [(1000, 260)]),                         # R = 8
+    # R = 4, 5, 3: 32, 25, 42 tokens per 128-row tile leave 0, 3, 2 padding rows; chunks starting mid-page
+    (32, 8, [(100, 300), (0, 70)]),
+    (40, 8, [(1000, 257), (37, 19)]),
+    (24, 8, [(197, 200), (64, 1)]),
 ])
 def test_prefill_attention_long_context_vs_fp32(cuda_device, kernel, n_q, n_kv, seqs):
     """Prefill attention alone (both kernels: wgmma `tc` / `tc2` = generation 1 / 2, mma.sync `mma`): chunks of queries at arbitrary positions

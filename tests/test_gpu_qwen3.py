@@ -19,35 +19,50 @@ def _inv_freq(dev, theta=1e6):
 
 
 # ---- token-step epilogue -------------------------------------------------------------------------------------------
-def _epilogue_case(dev, B, n_q, n_kv, n_split, seed, bias=True):
+def _epilogue_case(dev, B, n_q, n_kv, n_split, seed, bias=True, rope="hf"):
+    """rope "hf": Qwen's unscaled table, positions below 2 pages, token row b in block-table row b.  rope "llama3":
+    Llama-3.1-8B's scaled table, positions up to 131071, each row in a block-table row of its own (a permutation of more
+    rows than there are tokens) with one page at the block its position falls in."""
     g = torch.Generator().manual_seed(seed)
     nh = n_q + 2 * n_kv
-    P, max_blocks = 64, 8
-    n_pages = 1 + B * 2
+    P = 64
     part = (torch.randn(n_split, B, nh * D, generator=g) * 0.7).to(dev)
     b = (0.3 * torch.randn(nh * D, generator=g)).to(torch.bfloat16).to(dev) if bias else None
     qg = (1 + 0.4 * torch.randn(D, generator=g)).to(torch.bfloat16).to(dev)
     kg = (1 + 0.4 * torch.randn(D, generator=g)).to(torch.bfloat16).to(dev)
-    pos = torch.randint(0, 2 * P, (B,), generator=g, dtype=torch.int32)
-    bt = torch.zeros(B, max_blocks, dtype=torch.int32)
-    bt[:, :2] = (1 + torch.randperm(2 * B, generator=g)).view(B, 2).int()
-    return dict(part=part, bias=b, qg=qg, kg=kg, pos=pos.to(dev), bt=bt.to(dev), n_pages=n_pages, P=P,
-                max_blocks=max_blocks, B=B, n_q=n_q, n_kv=n_kv, n_split=n_split)
+    if rope == "hf":
+        max_blocks, n_pages = 8, 1 + B * 2
+        pos = torch.randint(0, 2 * P, (B,), generator=g, dtype=torch.int32)
+        slot = torch.arange(B, dtype=torch.int32)
+        bt = torch.zeros(B, max_blocks, dtype=torch.int32)
+        bt[:, :2] = (1 + torch.randperm(2 * B, generator=g)).view(B, 2).int()
+        inv = _inv_freq(dev)
+    else:
+        from pipelinerl_b200.model import ModelConfig, rope_inv_freq
+        max_blocks, n_pages = 131072 // P, 1 + B + 2                  # two pages no token addresses
+        pos = torch.randint(0, 131072, (B,), generator=g, dtype=torch.int32)
+        pos[:4] = torch.tensor([131071, 0, 63, 64], dtype=torch.int32)[:B]
+        slot = torch.randperm(B + 5, generator=g)[:B].int()
+        bt = torch.zeros(B + 5, max_blocks, dtype=torch.int32)
+        bt[slot.long(), (pos // P).long()] = (1 + torch.randperm(B, generator=g)).int()
+        inv = rope_inv_freq(ModelConfig.llama3_1_8b()).to(dev)
+    return dict(part=part, bias=b, qg=qg, kg=kg, pos=pos.to(dev), bt=bt.to(dev), slot=slot.to(dev), inv=inv,
+                n_pages=n_pages, P=P, max_blocks=max_blocks, B=B, n_q=n_q, n_kv=n_kv, n_split=n_split)
 
 
-def _run_epilogue(lib, c, dev, norm=True, rows=None, legacy=False, eps=1e-6, layer=1):
-    """-> (q_out [B, n_q, D], kv cache [2 layers, 2, n_pages, n_kv, P, D]); rows = (r0, n): only those token rows"""
+def _run_epilogue(lib, c, dev, norm=True, rows=None, legacy=False, eps=1e-6, layer=1, kv0=None):
+    """-> (q_out [B, n_q, D], kv cache [2 layers, 2, n_pages, n_kv, P, D]); rows = (r0, n): only those token rows; kv0: the
+    cache's contents before the step (zeros by default)"""
     from pipelinerl_b200 import _lib
     B, n_q, n_kv = c["B"], c["n_q"], c["n_kv"]
     q = torch.zeros(B, n_q, D, dtype=torch.bfloat16, device=dev)
-    kv = torch.zeros(2 * 2 * c["n_pages"] * n_kv * c["P"] * D, dtype=torch.bfloat16, device=dev)
-    inv = _inv_freq(dev)
+    kv = (kv0.clone() if kv0 is not None else
+          torch.zeros(2 * 2 * c["n_pages"] * n_kv * c["P"] * D, dtype=torch.bfloat16, device=dev))
     r0, n = rows if rows is not None else (0, B)
     assert c["n_split"] == 1 or rows is None
     part = c["part"][:, r0:r0 + n].contiguous()
     bias = c["bias"].data_ptr() if c["bias"] is not None else None
-    slot = torch.arange(r0, r0 + n, dtype=torch.int32, device=dev)
-    common = (c["pos"][r0:].data_ptr(), c["bt"].data_ptr(), c["max_blocks"], slot.data_ptr(), inv.data_ptr(),
+    common = (c["pos"][r0:].data_ptr(), c["bt"].data_ptr(), c["max_blocks"], c["slot"][r0:].data_ptr(), c["inv"].data_ptr(),
               q[r0:].data_ptr(), kv.data_ptr(), c["n_pages"], layer, c["P"], None, 0, None)
     if legacy:
         _lib.check(lib.prl_qkv_rope_cache(part.data_ptr(), c["n_split"], n, bias, n_q, n_kv, D, *common))
@@ -59,43 +74,72 @@ def _run_epilogue(lib, c, dev, norm=True, rows=None, legacy=False, eps=1e-6, lay
     return q, kv.view(2, 2, c["n_pages"], n_kv, c["P"], D)
 
 
-def _epilogue_fp64(c, eps=1e-6):
+def _epilogue_fp64(c, eps=1e-6, norm=True):
     x = c["part"].double().sum(0)
     if c["bias"] is not None:
         x = x + c["bias"].double()
     B, n_q, n_kv = c["B"], c["n_q"], c["n_kv"]
     x = x.view(B, n_q + 2 * n_kv, D)
-    qk = x[:, :n_q + n_kv]
-    gam = torch.cat([c["qg"].double()[None].expand(n_q, D), c["kg"].double()[None].expand(n_kv, D)])
-    y = qk * torch.rsqrt((qk * qk).mean(-1, keepdim=True) + eps) * gam
-    ang = (c["pos"].float()[:, None] * _inv_freq(c["pos"].device)[None]).double()   # the kernel's fp32 angle
+    y = x[:, :n_q + n_kv]
+    if norm:
+        gam = torch.cat([c["qg"].double()[None].expand(n_q, D), c["kg"].double()[None].expand(n_kv, D)])
+        y = y * torch.rsqrt((y * y).mean(-1, keepdim=True) + eps) * gam
+    ang = (c["pos"].float()[:, None] * c["inv"][None]).double()       # the kernel's fp32 angle
     cs, sn = torch.cos(ang)[:, None], torch.sin(ang)[:, None]
     y1, y2 = y[..., :64], y[..., 64:]
     return torch.cat([y1 * cs - y2 * sn, y2 * cs + y1 * sn], -1), x[:, n_q + n_kv:]
 
 
+def _kv_page_slot(c):
+    """page and in-page slot of every token row's KV"""
+    pos = c["pos"].long()
+    return c["bt"].long()[c["slot"].long(), pos // c["P"]], pos % c["P"]
+
+
 def _kv_rows(c, kv, layer=1):
     """k [B, n_kv, D], v [B, n_kv, D] of every token row, read back from the pages"""
-    P = c["P"]
-    pos = c["pos"].long()
-    page = c["bt"].long().gather(1, (pos // P)[:, None])[:, 0]
-    slot = pos % P
+    page, slot = _kv_page_slot(c)
     return kv[layer, 0, page, :, slot], kv[layer, 1, page, :, slot]
 
 
-@pytest.mark.parametrize("B,n_q,n_kv,n_split", [(5, 8, 2, 3), (64, 32, 8, 2), (300, 8, 2, 1), (200, 5, 1, 1)])
-def test_qkv_norm_rope_epilogue_vs_fp64(cuda_device, B, n_q, n_kv, n_split):
-    """per-head kernel (B <= 128) and row-walking kernel (B > 128) against an fp64 restatement: one bf16 rounding"""
+def _case(B, n_q, n_kv, n_split, norm=True, bias=True, rope="hf"):
+    tag = "-".join(map(str, (B, n_q, n_kv, n_split))) + ("" if norm else "-nonorm") + ("" if bias else "-nobias")
+    return pytest.param(B, n_q, n_kv, n_split, norm, bias, rope, id=tag + ("" if rope == "hf" else "-" + rope))
+
+
+@pytest.mark.parametrize("B,n_q,n_kv,n_split,norm,bias,rope", [
+    _case(5, 8, 2, 3), _case(64, 32, 8, 2), _case(300, 8, 2, 1), _case(200, 5, 1, 1),
+    # the Qwen2 step (bias, no q/k norm) on both kernels; Qwen3 (norm, no bias) at Qwen3-8B's and Qwen3-14B's groupings
+    _case(5, 28, 4, 3, norm=False), _case(300, 28, 4, 1, norm=False),
+    _case(64, 32, 8, 2, bias=False), _case(129, 40, 8, 1, bias=False),
+    # the Llama 3 step (neither) with the scaled table, positions up to 131071 and scattered block-table rows
+    _case(7, 32, 8, 2, norm=False, bias=False, rope="llama3"), _case(200, 24, 8, 2, norm=False, bias=False, rope="llama3"),
+    _case(150, 8, 2, 1, bias=False, rope="llama3"),
+])
+def test_qkv_norm_rope_epilogue_vs_fp64(cuda_device, B, n_q, n_kv, n_split, norm, bias, rope):
+    """per-head kernel (B <= 128) and row-walking kernel (B > 128) against an fp64 restatement: one bf16 rounding.  The
+    cache starts out holding a pattern, and every row the step does not address must still hold it afterwards."""
     from pipelinerl_b200 import _lib
     lib = _lib.load()
-    c = _epilogue_case(cuda_device, B, n_q, n_kv, n_split, seed=B + n_q)
-    q, kv = _run_epilogue(lib, c, cuda_device)
-    qk_ref, v_ref = _epilogue_fp64(c)
+    c = _epilogue_case(cuda_device, B, n_q, n_kv, n_split, seed=B + n_q, bias=bias, rope=rope)
+    kv0 = torch.randn(2 * 2 * c["n_pages"] * n_kv * c["P"] * D, generator=torch.Generator().manual_seed(1))
+    kv0 = kv0.to(torch.bfloat16).to(cuda_device)
+    q, kv = _run_epilogue(lib, c, cuda_device, norm=norm, kv0=kv0)
+    qk_ref, v_ref = _epilogue_fp64(c, norm=norm)
     k, v = _kv_rows(c, kv)
-    got = torch.cat([q, k], 1).double()
+    got = torch.cat([q, k], 1)
     tol = 2 ** -7 * qk_ref.abs() + 1e-5            # one bf16 rounding (a boundary case may round the other way)
-    assert ((got - qk_ref).abs() <= tol).all(), (got - qk_ref).abs().max().item()
+    err = (got.double() - qk_ref).abs()
+    exact = (got == qk_ref.to(torch.bfloat16)).double().mean().item()
+    print(f"[qkv epilogue {B}x{n_q}/{n_kv} split {n_split} norm {norm} bias {bias} rope {rope}] max |err| "
+          f"{err.max().item():.3e}, exact {exact:.5f}")
+    assert (err <= tol).all(), err.max().item()
+    assert exact >= 0.999, exact
     assert ((v.double() - v_ref).abs() <= 2 ** -7 * v_ref.abs() + 1e-5).all()   # v heads: sum + bias only, no norm
+    page, slot = _kv_page_slot(c)
+    written = torch.zeros(2, 2, c["n_pages"], n_kv, c["P"], dtype=torch.bool, device=cuda_device)
+    written[1, :, page, :, slot] = True
+    assert torch.equal(kv[~written], kv0.view_as(kv)[~written])
 
 
 def test_qkv_norm_rope_rows_kernel_bit_identical_to_per_head_kernel(cuda_device):
