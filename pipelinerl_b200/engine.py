@@ -365,14 +365,14 @@ class DecodeEngine:
                 _lib.check(lib.prl_residual_rmsnorm(part.data_ptr(), self.split_k["down"], B, H, a.ptr(nxt), cfg.rms_eps,
                                                     self.h.data_ptr(), self.x.data_ptr(), None, 0, st))
         if not self.fused_head:
-            self._gemm("lm_head.weight", self.x, cfg.head_rows, H, 1, self.logits,
+            self._gemm(cfg.head_name, self.x, cfg.head_rows, H, 1, self.logits,
                        lo="lm_head.weight_lo" if cfg.fp32_head else None)
 
     def _sample_and_advance(self) -> None:
         lib, st = self.lib, _lib.stream_ptr()
         if self.fused_head:
             cfg, a = self.cfg, self.arena
-            _lib.check(lib.prl_head_logprob(a.ptr("lm_head.weight"), a.ptr("lm_head.weight_lo") if cfg.fp32_head else None,
+            _lib.check(lib.prl_head_logprob(a.ptr(cfg.head_name), a.ptr("lm_head.weight_lo") if cfg.fp32_head else None,
                                             self.x.data_ptr(), self.B, cfg.vocab_size, cfg.hidden_size,
                                             float(self.temperature), None, int(self.greedy), self.seed, self.step_count,
                                             None, None, None, self.sampled.data_ptr(), self.sampled_lp.data_ptr(),
@@ -563,7 +563,7 @@ class DecodeEngine:
             pf["head_ws"] = torch.zeros(int(lib.prl_head_workspace_bytes(self.prefill_chunk, cfg.vocab_size)),
                                         dtype=torch.uint8, device=self.dev)
         pf["targets"][:n].copy_(torch.tensor(tg, dtype=torch.int64), non_blocking=True)
-        _lib.check(lib.prl_head_logprob(a.ptr("lm_head.weight"), a.ptr("lm_head.weight_lo") if cfg.fp32_head else None,
+        _lib.check(lib.prl_head_logprob(a.ptr(cfg.head_name), a.ptr("lm_head.weight_lo") if cfg.fp32_head else None,
                                         x.data_ptr(), n, cfg.vocab_size, H, float(score_temperature),
                                         pf["targets"].data_ptr(), 1, 0, 0, pf["lp"].data_ptr(), None, None, None, None,
                                         pf["head_ws"].data_ptr(), pf["head_ws"].numel(), st))

@@ -64,7 +64,8 @@ def hf_config_dict(cfg: ModelConfig) -> dict[str, Any]:
                 "num_key_value_heads": cfg.num_kv_heads, "head_dim": cfg.head_dim, "hidden_act": "silu",
                 "rms_norm_eps": cfg.rms_eps, "rope_theta": cfg.rope_theta,
                 "rope_scaling": cfg.rope_scaling.hf_dict() if cfg.rope_scaling is not None else None,
-                "tie_word_embeddings": False, "torch_dtype": "bfloat16", "attention_bias": False, "mlp_bias": False}
+                "tie_word_embeddings": cfg.tie_word_embeddings, "torch_dtype": "bfloat16", "attention_bias": False,
+                "mlp_bias": False}
     if cfg.qk_norm:
         d = {"architectures": ["Qwen3ForCausalLM"], "model_type": "qwen3"}
     else:
@@ -72,8 +73,8 @@ def hf_config_dict(cfg: ModelConfig) -> dict[str, Any]:
     d.update({"vocab_size": cfg.vocab_size,
               "hidden_size": cfg.hidden_size, "intermediate_size": cfg.intermediate_size, "num_hidden_layers": cfg.num_layers,
               "num_attention_heads": cfg.num_q_heads, "num_key_value_heads": cfg.num_kv_heads, "head_dim": cfg.head_dim,
-              "hidden_act": "silu", "rms_norm_eps": cfg.rms_eps, "rope_theta": cfg.rope_theta, "tie_word_embeddings": False,
-              "torch_dtype": "bfloat16"})
+              "hidden_act": "silu", "rms_norm_eps": cfg.rms_eps, "rope_theta": cfg.rope_theta,
+              "tie_word_embeddings": cfg.tie_word_embeddings, "torch_dtype": "bfloat16"})
     if not cfg.qk_norm:
         d["attention_bias"] = cfg.qkv_bias
     elif cfg.qkv_bias:      # Qwen3Config's default is False
@@ -90,7 +91,8 @@ def _hf_tensors(cfg: ModelConfig, fused: dict[str, torch.Tensor]) -> dict[str, t
 
 
 def save_model_only(output_dir: Path, cfg: ModelConfig, named_parameters, dtype: torch.dtype = torch.bfloat16) -> None:
-    """`named_parameters`: (fused name, tensor) pairs -- a learner module's named_parameters() or an arena's views."""
+    """`named_parameters`: (fused name, tensor) pairs -- a learner module's named_parameters() or an arena's views.  A
+    tied config writes no `lm_head.weight` (config.json says tie_word_embeddings), as HF saves a tied model."""
     from safetensors.torch import save_file
     fused = {n: (p.data if hasattr(p, "data") else p).to(dtype) for n, p in named_parameters}
     with get_temporary_folder_and_move(Path(output_dir)) as tmp:

@@ -69,7 +69,7 @@ class TorchQwen2(torch.nn.Module):
         hidden = self.hidden_states(batch.input_ids, batch.position_ids if batch.is_packed else None)
         lps, ents = [], []
         for b in range(hidden.shape[0]):
-            lp, ent = fused_head_logprobs(hidden[b, :-1], self.p("lm_head.weight"), batch.input_ids[b, 1:], temperature)
+            lp, ent = fused_head_logprobs(hidden[b, :-1], self.p(self.cfg.head_name), batch.input_ids[b, 1:], temperature)
             lps.append(lp)
             ents.append(ent)
         return torch.stack(lps), torch.stack(ents)
@@ -78,7 +78,7 @@ class TorchQwen2(torch.nn.Module):
         """Packed rows [1, T] with position_ids restarting per sample (block-diagonal causal attention), or
         padded [B, L] batches."""
         x = self.hidden_states(input_ids, position_ids)
-        return types.SimpleNamespace(logits=F.linear(x.float(), self.p("lm_head.weight").float()))
+        return types.SimpleNamespace(logits=F.linear(x.float(), self.p(self.cfg.head_name).float()))
 
     def hidden_states(self, input_ids, position_ids=None):
         """Final-norm hidden states [B, T, H]."""
@@ -130,7 +130,7 @@ class _NativeHead(torch.autograd.Function):
     def forward(ctx, hidden, model, targets, temperature: float, chunk_rows: int):
         lib = _lib.load()
         x = hidden.to(torch.bfloat16).contiguous()
-        W = model.p("lm_head.weight").data
+        W = model.p(model.cfg.head_name).data
         M, K = x.shape
         V = W.shape[0]
         tg = targets.to(torch.int64).contiguous()
@@ -152,7 +152,9 @@ class _NativeHead(torch.autograd.Function):
         model, lib = ctx.model, _lib.load()
         body = model.body
         ops = body.ops
-        W, gW = model.p("lm_head.weight").data, body.g["lm_head.weight"]
+        # tied: W is the embedding table and gW its gradient view, into which NativeBody.backward's embedding
+        # scatter-add later accumulates the other use (nothing zeroes the gradient arena in between)
+        W, gW = model.p(model.cfg.head_name).data, body.g[model.cfg.head_name]
         M, K = x.shape
         V = W.shape[0]
         dev = x.device
@@ -282,4 +284,4 @@ class NativeQwen2(torch.nn.Module):
 
     def forward(self, input_ids, attention_mask=None, labels=None, position_ids=None, **kw):
         x = self.hidden_states(input_ids, position_ids)
-        return types.SimpleNamespace(logits=F.linear(x.float(), self.p("lm_head.weight").float()))
+        return types.SimpleNamespace(logits=F.linear(x.float(), self.p(self.cfg.head_name).float()))

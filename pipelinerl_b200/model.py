@@ -48,6 +48,13 @@ class ModelConfig:
     lm_head_rows: int | None = None  # vocabulary rows of THIS shard's lm_head (vocab-parallel head under TP)
     family: str = "qwen"     # "qwen" (Qwen2 / Qwen3, told apart by qk_norm) or "llama": the config.json a checkpoint gets
     rope_scaling: Llama3RopeScaling | None = None   # None: plain RoPE, inv_freq = 1 / theta^(2i / d)
+    tie_word_embeddings: bool = False  # one [V, H] table is both the input embedding and the head (no lm_head tensor)
+
+    def __post_init__(self):
+        if self.tie_word_embeddings and self.fp32_head:
+            raise ValueError("fp32_head=True with tie_word_embeddings=True: a tied head is the bf16 embedding table, and "
+                             "its logits are already computed as the reference computes a tied head, fp32 accumulation "
+                             "over the bf16 table (the head kernels with W_lo = NULL); drop fp32_head")
 
     @property
     def q_size(self) -> int:
@@ -60,6 +67,11 @@ class ModelConfig:
     @property
     def qkv_size(self) -> int:
         return self.q_size + 2 * self.kv_size
+
+    @property
+    def head_name(self) -> str:
+        """Arena name of the tensor the head reads: the embedding table when the word embeddings are tied."""
+        return "embed_tokens.weight" if self.tie_word_embeddings else "lm_head.weight"
 
     @property
     def head_rows(self) -> int:
@@ -85,7 +97,8 @@ class ModelConfig:
 
     @staticmethod
     def qwen2_5_1_5b(**kw) -> "ModelConfig":
-        """Qwen2.5-1.5B's shapes (its input and output embeddings are stored untied here)."""
+        """Qwen2.5-1.5B's shapes (its checkpoint ties the word embeddings; pass tie_word_embeddings=True to train them
+        tied, the default stores an untied copy of the head)."""
         return ModelConfig(vocab_size=151936, hidden_size=1536, intermediate_size=8960, num_layers=28,
                            num_q_heads=12, num_kv_heads=2, **kw)
 
@@ -99,6 +112,13 @@ class ModelConfig:
         """Qwen3-8B's shapes (keyword arguments override, e.g. num_layers for a bounded sample of layers)."""
         base = dict(vocab_size=151936, hidden_size=4096, intermediate_size=12288, num_layers=36, num_q_heads=32,
                     num_kv_heads=8, qkv_bias=False, qk_norm=True)
+        return ModelConfig(**{**base, **kw})
+
+    @staticmethod
+    def qwen3_1_7b(**kw) -> "ModelConfig":
+        """Qwen3-1.7B's shapes, word embeddings tied as in its published config.json."""
+        base = dict(vocab_size=151936, hidden_size=2048, intermediate_size=6144, num_layers=28, num_q_heads=16,
+                    num_kv_heads=8, qkv_bias=False, qk_norm=True, tie_word_embeddings=True)
         return ModelConfig(**{**base, **kw})
 
     @staticmethod
@@ -117,16 +137,18 @@ class ModelConfig:
 
     @staticmethod
     def llama3_2_3b(**kw) -> "ModelConfig":
-        """Llama-3.2-3B(-Instruct)'s shapes and RoPE scaling (its tied embeddings are stored untied here)."""
+        """Llama-3.2-3B(-Instruct)'s shapes and RoPE scaling (its checkpoint ties the word embeddings; the default stores an
+        untied copy of the head, tie_word_embeddings=True trains them tied)."""
         base = dict(vocab_size=128256, hidden_size=3072, intermediate_size=8192, num_layers=28, num_q_heads=24,
                     num_kv_heads=8, rope_theta=500_000.0, rms_eps=1e-5, qkv_bias=False, family="llama",
                     rope_scaling=Llama3RopeScaling(32.0, 1.0, 4.0, 8192))
         return ModelConfig(**{**base, **kw})
 
     @staticmethod
-    def from_hf_config(d: dict) -> "ModelConfig":
+    def from_hf_config(d: dict, keep_tied: bool = False) -> "ModelConfig":
         """ModelConfig of an HF `config.json` dict of model_type "qwen2", "qwen3" (dense) or "llama" (Llama 3).  Tied
-        word embeddings are accepted: the arena keeps an untied copy of the head (ParamArena.load_hf_state_dict)."""
+        word embeddings are accepted: by default the arena keeps an untied copy of the head
+        (ParamArena.load_hf_state_dict); with keep_tied, `tie_word_embeddings` follows `d` and one table serves both."""
         mt = d.get("model_type")
         if mt not in ("qwen2", "qwen3", "llama"):
             raise ValueError(f"unsupported model_type {mt!r}: only 'qwen2', 'qwen3' (dense) and 'llama' are implemented")
@@ -142,6 +164,8 @@ class ModelConfig:
                       intermediate_size=int(d["intermediate_size"]), num_layers=int(d["num_hidden_layers"]),
                       num_q_heads=heads, num_kv_heads=int(d.get("num_key_value_heads", heads)), head_dim=head_dim,
                       rms_eps=float(d.get("rms_norm_eps", 1e-6)))
+        if keep_tied:
+            common["tie_word_embeddings"] = bool(d.get("tie_word_embeddings", False))
         if mt == "llama":
             return ModelConfig(**common, **_llama_fields(d))
         theta = d.get("rope_theta", rope.get("rope_theta", 1_000_000.0))
@@ -229,6 +253,8 @@ def fused_shapes(cfg: ModelConfig) -> list[tuple[str, tuple[int, ...]]]:
         out.append((p + "down_proj.weight", (H, I)))
     out.append(("embed_tokens.weight", (cfg.vocab_size, H)))
     out.append(("norm.weight", (H,)))
+    if cfg.tie_word_embeddings:
+        return out
     out.append(("lm_head.weight", (cfg.head_rows, H)))
     if cfg.fp32_head:
         out.append(("lm_head.weight_lo", (cfg.head_rows, H)))
@@ -274,7 +300,8 @@ class ArenaLayout:
             m[hp + "mlp.down_proj.weight"] = (fp + "down_proj.weight", 0, c.hidden_size)
         m["model.embed_tokens.weight"] = ("embed_tokens.weight", 0, c.vocab_size)
         m["model.norm.weight"] = ("norm.weight", 0, c.hidden_size)
-        m["lm_head.weight"] = ("lm_head.weight", 0, c.vocab_size)
+        if not c.tie_word_embeddings:
+            m["lm_head.weight"] = ("lm_head.weight", 0, c.vocab_size)
         return m
 
 
@@ -324,7 +351,16 @@ class ParamArena:
         return self
 
     def load_hf_state_dict(self, sd: dict[str, torch.Tensor]) -> None:
+        """HF-named tensors -> the arena.  A tied config takes a state dict with or without `lm_head.weight`; one that
+        has it must hold the embedding table there, or the checkpoint is not tied."""
         slices = self.layout.hf_slices()
+        if self.cfg.tie_word_embeddings and "lm_head.weight" in sd:
+            sd = dict(sd)
+            head = sd.pop("lm_head.weight")
+            emb = sd.get("model.embed_tokens.weight")
+            if emb is None or not torch.equal(head, emb):
+                raise ValueError("tie_word_embeddings=True but the state dict's lm_head.weight differs from "
+                                 "model.embed_tokens.weight: the checkpoint is not tied")
         seen = set()
         for hf_name, t in sd.items():
             if hf_name not in slices:

@@ -38,6 +38,9 @@ class TPDecodeEngine(DecodeEngine):
                                       "use DecodeEngine")
         if full_cfg.rope_scaling is not None:
             raise NotImplementedError("TPDecodeEngine does not implement RoPE scaling yet (Llama 3): use DecodeEngine")
+        if full_cfg.tie_word_embeddings:
+            raise NotImplementedError("TPDecodeEngine does not implement tied word embeddings (a vocab-parallel head over "
+                                      "the replicated embedding table): use DecodeEngine")
         if tp_size < 2 or tp_size > 8:
             raise ValueError("TPDecodeEngine is for 2..8 ranks; use DecodeEngine for tp=1")
         self.full_cfg, self.tp_rank, self.tp, self.dist, self.group = full_cfg, tp_rank, tp_size, dist, group
@@ -125,7 +128,7 @@ class TPDecodeEngine(DecodeEngine):
             _lib.check(lib.prl_silu_mul(part.data_ptr(), self.split_k["gate_up"], B, I, self.act.data_ptr(), None, 0, st))
             nxt = f"layers.{l + 1}.input_layernorm.weight" if l + 1 < cfg.num_layers else "norm.weight"
             self._row_parallel(p + "down_proj.weight", self.act, H, I, 1, s_dense, 2 * l + 2, a.ptr(nxt))
-        self._gemm("lm_head.weight", self.x, cfg.head_rows, H, 1, self.logits)
+        self._gemm(cfg.head_name, self.x, cfg.head_rows, H, 1, self.logits)
 
     def step(self) -> None:
         """Like DecodeEngine.step, but the base class's eager warm-up before graph capture would deliver every
