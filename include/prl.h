@@ -565,6 +565,40 @@ typedef struct {
 } prl_engine_state;
 int prl_advance_state(const prl_engine_state* state, prl_stream_t stream);
 
+/* Stop strings and min_tokens for the state advance, in a struct of their own so that prl_engine_state keeps its
+ * layout.  prl_advance_state_strings(state, strings) is prl_advance_state plus these rules; with every pointer of
+ * `strings` NULL it is prl_advance_state bit for bit. */
+typedef struct {
+  /* stop strings (vLLM's `stop`), matched on the bytes the detokenizer emits, after the rules above: a KMP automaton
+   * per (slot, string) advances over the token's bytes; the first string in the slot's order whose match ends inside
+   * this token finishes the slot with finished=1, whatever the rules above decided.  The token that ended the slot on
+   * eos or a stop id is fed only with the "include stop string" flag; a special token contributes no bytes with the
+   * "skip special tokens" flag.  With tok_bytes == NULL none of the string fields is read. */
+  const uint8_t* tok_bytes;        /* bytes of every token id, concatenated */
+  const int32_t* tok_offsets;      /* [vocab + 1] token t is tok_bytes[tok_offsets[t] .. tok_offsets[t+1]) */
+  const uint8_t* tok_special;      /* [vocab] 1: special token */
+  int32_t vocab;
+  const uint8_t* stop_str;         /* [B, max_stop_str, stop_str_stride] the strings' bytes */
+  const int16_t* stop_str_fail;    /* [B, max_stop_str, stop_str_stride] KMP failure function of each string */
+  const int32_t* stop_str_len;     /* [B, max_stop_str] bytes per string (1..stop_str_stride) */
+  const int32_t* n_stop_str;       /* [B] strings used in each row (0..max_stop_str) */
+  int32_t max_stop_str;
+  int32_t stop_str_stride;
+  const uint8_t* stop_str_flags;   /* [B] bit 0: include the stop string in the output; bit 1: skip special tokens */
+  int32_t* stop_str_state;         /* [B, max_stop_str] matcher state (matched prefix length), zeroed at admission */
+  int32_t* stop_str_match;         /* [B] written when a slot finishes: index of the string that ended it, else -1 */
+  /* vLLM's min_tokens: while a slot holds fewer outputs than this, neither the rules above nor the strings end it */
+  const int32_t* min_tokens;       /* [B] or NULL (0 for every slot) */
+} prl_stop_strings;
+int prl_advance_state_strings(const prl_engine_state* state, const prl_stop_strings* strings, prl_stream_t stream);
+
+/* min_tokens logit ban (vLLM's MinTokensLogitsProcessor): for every row b with gen_count[b] < min_tokens[b], sets
+ * logits[b, id] = -inf for each of the n_ban[b] ids of ban_ids[b, :] (ids outside [0, V) are skipped).  Runs between
+ * the head GEMM and the sampler, so the sampled id and its processed logprob are those of the masked distribution. */
+int prl_ban_min_tokens(float* logits /*[B,V]*/, int32_t B, int32_t V, const int32_t* gen_count, const int32_t* min_tokens,
+                       const int32_t* ban_ids /*[B, ban_stride]*/, int32_t ban_stride, const int32_t* n_ban,
+                       prl_stream_t stream);
+
 /* ---- tensor parallelism inside one engine (BASELINE config 4: Qwen2.5-32B, TP=2; the reference passes
  * tensor-parallel-size to vLLM, world.py:56-59, which all-reduces twice per layer with NCCL/custom all-reduce).
  * Here the row-parallel GEMMs (o_proj, down_proj) store their fp32 partial tiles into the local AND the peer GPU's

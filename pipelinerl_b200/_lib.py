@@ -80,6 +80,15 @@ class EngineState(C.Structure):
     ]
 
 
+class StopStrings(C.Structure):
+    _fields_ = [
+        ("tok_bytes", C.c_void_p), ("tok_offsets", C.c_void_p), ("tok_special", C.c_void_p), ("vocab", C.c_int32),
+        ("stop_str", C.c_void_p), ("stop_str_fail", C.c_void_p), ("stop_str_len", C.c_void_p), ("n_stop_str", C.c_void_p),
+        ("max_stop_str", C.c_int32), ("stop_str_stride", C.c_int32), ("stop_str_flags", C.c_void_p),
+        ("stop_str_state", C.c_void_p), ("stop_str_match", C.c_void_p), ("min_tokens", C.c_void_p),
+    ]
+
+
 class MbRecord(C.Structure):
     _fields_ = [("n_chunk", C.c_int32), ("n_pack", C.c_int32), ("padding", C.c_int32), ("total_tok", C.c_int32),
                 ("total_lp", C.c_int32), ("n_stat_slots", C.c_int32), ("n_rollout_slots", C.c_int32), ("n_groups", C.c_int32),
@@ -223,6 +232,9 @@ _SIGNATURES = {
                                                 C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "prl_advance_state": (C.c_int, [C.POINTER(EngineState), C.c_void_p]),
+    "prl_advance_state_strings": (C.c_int, [C.POINTER(EngineState), C.POINTER(StopStrings), C.c_void_p]),
+    "prl_ban_min_tokens": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                     C.c_void_p, C.c_void_p]),
     "prl_gemm_bf16_splitk_peer": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
                                             C.c_void_p, C.c_void_p, C.c_void_p]),
     "prl_tp_signal": (C.c_int, [C.c_void_p, C.c_void_p]),

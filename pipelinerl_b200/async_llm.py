@@ -2,7 +2,8 @@
 (reference: pipelinerl/async_llm.py:86-212 and :215-346)."""
 from __future__ import annotations
 
-from .engine import SamplingParams, requested_truncation, stop_token_ids_param, truncation_params
+from .engine import (SamplingParams, check_stop_flags, min_tokens_param, requested_truncation, stop_strings_param,
+                     stop_token_ids_param, truncation_params)
 from .llm import LLMCall, LLMOutput, Prompt, TokenLogprob, TrainableLLM
 from .rollouts import TrainingText, apply_rollout_reward
 from .serving import resolve, sampling_features
@@ -39,7 +40,8 @@ def _reject_unsupported_sampling(params: dict, features: frozenset = frozenset()
     a silently ignored top_p / top_k / stop would make the recorded logprobs those of a different distribution than the
     one the request asked for.  top_k / top_p are accepted when the target engine lists them in `features` (the unfused
     single-GPU DecodeEngine does; the reference's eval handles send top_p 0.95 / top_k 50, conf/base.yaml:52-57), and
-    stop_token_ids when it lists "stop_token_ids"; they are validated as vLLM validates them.  Stop strings are refused.
+    stop_token_ids when it lists "stop_token_ids"; they are validated as vLLM validates them.  Stop strings and
+    min_tokens > 0 are refused unless it lists "stop" / "min_tokens" (stop_params validates them).
     Returns the request's (top_k, top_p, stop_token_ids)."""
     greedy = float(params.get("temperature", 1.0)) <= 0
     top_k, top_p = truncation_params(params, greedy=greedy)
@@ -49,7 +51,7 @@ def _reject_unsupported_sampling(params: dict, features: frozenset = frozenset()
     stop_ids = stop_token_ids_param(params)
     if stop_ids and "stop_token_ids" not in features:
         raise ValueError("stop token ids are not implemented by this engine (eos only)")
-    if params.get("stop"):
+    if stop_strings_param(params) and "stop" not in features:
         raise ValueError("stop strings are not implemented by this engine (stop token ids are)")
     if int(params.get("n", 1)) != 1:
         raise ValueError("n > 1 completions per request is not implemented (the actor issues `attempts` requests)")
@@ -57,6 +59,25 @@ def _reject_unsupported_sampling(params: dict, features: frozenset = frozenset()
         if params.get(name) not in (None, 0, 0.0, 1, 1.0) or (name == "repetition_penalty" and params.get(name) not in (None, 1, 1.0)):
             raise ValueError(f"sampling parameter {name} is not implemented by this engine")
     return top_k, top_p, stop_ids
+
+
+def stop_params(params: dict, features: frozenset, max_tokens: int,
+                collect_logprobs: bool) -> tuple[tuple[str, ...], int, bool, bool]:
+    """(stop, min_tokens, include_stop_str_in_output, skip_special_tokens) of a request.  The flags are what the
+    reference's client sends: (True, False) when it collects logprobs, else whatever `params` says, vLLM's defaults
+    (False, True) when it says nothing; with stop strings, a mixed pair is refused.  min_tokens > 0 is refused unless
+    the engine lists "min_tokens".  Raises ValueError."""
+    stop = stop_strings_param(params)
+    min_tokens = min_tokens_param(params, max_tokens)
+    if min_tokens and "min_tokens" not in features:
+        raise ValueError("min_tokens is not implemented by this engine")
+    if collect_logprobs:
+        include, skip = True, False
+    else:
+        include = bool(params.get("include_stop_str_in_output", False))
+        skip = bool(params.get("skip_special_tokens", True))
+    check_stop_flags(stop, include, skip)
+    return stop, min_tokens, include, skip
 
 
 async def llm_async_generate(llm: TrainableLLM, prompt: Prompt, session=None,
@@ -68,17 +89,23 @@ async def llm_async_generate(llm: TrainableLLM, prompt: Prompt, session=None,
     prompt_ids = prompt.token_ids or _token_ids(tok.apply_chat_template(prompt.messages, add_generation_prompt=True,
                                                                         **_chat_kwargs(llm, prompt)))
     params = llm.parameters
-    top_k, top_p, stop_ids = _reject_unsupported_sampling(params, sampling_features(llm.base_url))
+    features = sampling_features(llm.base_url)
+    top_k, top_p, stop_ids = _reject_unsupported_sampling(params, features)
     max_tokens = int(max_tokens_override if max_tokens_override is not None else params.get("max_tokens", 16))
+    stop, min_tokens, include, skip = stop_params(params, features, max_tokens, bool(llm.collect_logprobs))
     temperature = float(params.get("temperature", 1.0))
     sp = SamplingParams(max_tokens=max_tokens, temperature=temperature if temperature > 0 else 1.0,
                         greedy=temperature <= 0, ignore_eos=bool(params.get("ignore_eos", False)), top_k=top_k,
-                        top_p=top_p, stop_token_ids=stop_ids)
+                        top_p=top_p, stop_token_ids=stop_ids, stop=stop, min_tokens=min_tokens,
+                        include_stop_str_in_output=include, skip_special_tokens=skip)
     server = resolve(llm.base_url)
     if stop_ids:
         server.engine.stop_row(sp)      # out-of-vocabulary ids or too many: ValueError here, not on the engine thread
+    if stop:
+        server.engine.stop_string_rows(sp)   # past the engine's row limits: ValueError here as well
     req = await server.generate(list(prompt_ids), sp)
-    content = tok.decode(req.output_ids)
+    # with stop strings the content is vLLM's output_text (cut at the string), which the engine computed
+    content = req.output_text if stop and getattr(req, "output_text", None) is not None else tok.decode(req.output_ids)
     call = llm.log_output(prompt, LLMOutput(content=content), count_tokens=False)
     call.prompt_length_tokens = len(prompt_ids)
     call.output_length_tokens = len(req.output_ids)

@@ -358,7 +358,8 @@ __global__ void __launch_bounds__(kSampleThreads) sample_partial_kernel(const fl
   float best_z = 0.f;
   for (int i = lo + threadIdx.x; i < hi; i += kSampleThreads) {
     const float zi = z[i] * inv_temp;
-    if (zi > m) { s = s * __expf(m - zi) + 1.f; m = zi; } else { s += __expf(zi - m); }
+    // a -inf logit (a min_tokens ban) adds nothing; guarded, as __expf(-inf - -inf) would be NaN
+    if (zi > m) { s = s * __expf(m - zi) + 1.f; m = zi; } else if (zi != -INFINITY) { s += __expf(zi - m); }
     const int gid = vocab_offset + i;   // global vocabulary id (vocab-parallel head: this rank owns a slice)
     const float key = greedy ? zi : zi + gumbel(seed, step, (uint32_t)b, (uint32_t)gid);
     const ArgMax cand{key, gid};
@@ -456,11 +457,51 @@ __global__ void tp_epoch_kernel(unsigned long long* epoch) {
   if (threadIdx.x == 0) *epoch += 1ull;
 }
 
+// ---- stop strings: vLLM's IncrementalDetokenizer.update + check_stop_strings, on bytes ------------------------------
+// The detokenizer appends the token's text and looks for the first string, in request order, with an occurrence that
+// ends inside the new text.  On bytes that is: the string whose KMP automaton completes a match while it consumes this
+// token's bytes (a UTF-8 string can only match at character boundaries, and a character completes with its last
+// byte).  Tokens up to min_tokens are fed, so a match may start inside them, but they never report (`checked` false).
+// The automaton state of each (slot, string) is the length of the longest prefix of the string that ends the bytes fed
+// so far; no text is kept.  Returns the index of the matching string, or -1.
+__device__ __forceinline__ int match_stop_strings(const prl_stop_strings& st, int b, int id, bool core_stop,
+                                                  bool checked) {
+  const int ns = min(st.n_stop_str[b], st.max_stop_str);
+  if (ns <= 0 || id < 0 || id >= st.vocab) return -1;
+  const uint8_t flags = st.stop_str_flags[b];
+  // include_stop_str_in_output=False: the eos / stop id that ended the request is not detokenized
+  if (core_stop && !(flags & 1)) return -1;
+  // skip_special_tokens=True: a special token's text is empty
+  if ((flags & 2) && st.tok_special[id]) return -1;
+  const uint8_t* bytes = st.tok_bytes + st.tok_offsets[id];
+  const int nb = st.tok_offsets[id + 1] - st.tok_offsets[id];
+  const int64_t row = (int64_t)b * st.max_stop_str;
+  for (int j = 0; j < ns; ++j) {
+    const uint8_t* s = st.stop_str + (row + j) * st.stop_str_stride;
+    const int16_t* fail = st.stop_str_fail + (row + j) * st.stop_str_stride;
+    const int len = st.stop_str_len[row + j];
+    int q = st.stop_str_state[row + j];
+    bool hit = false;
+    for (int i = 0; i < nb; ++i) {
+      const uint8_t c = bytes[i];
+      while (q > 0 && s[q] != c) q = fail[q - 1];
+      if (s[q] == c) ++q;
+      if (q == len) {
+        hit = true;
+        q = fail[len - 1];
+      }
+    }
+    st.stop_str_state[row + j] = q;
+    if (hit && checked) return j;  // the slot finishes: the later strings' states are not needed any more
+  }
+  return -1;
+}
+
 // ---- advance the per-sequence state after a step (device-side, no host round trip) -------------
 // Slot b just processed the token at position pos.  While the next position is still inside the
 // prompt the sample is discarded and the next prompt token is fed (prefill-by-decode); afterwards
 // the sampled id / logprob are appended to the slot's output ring and become the next input.
-__global__ void advance_kernel(prl_engine_state st) {
+__global__ void advance_kernel(prl_engine_state st, prl_stop_strings ss) {
   pdl_launch_dependents();
   pdl_wait();
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -478,12 +519,15 @@ __global__ void advance_kernel(prl_engine_state st) {
     st.gen_count[b] = n + 1;
     st.tokens[b] = id;
     const bool ignore = st.ignore_eos || (st.ignore_eos_rows != nullptr && st.ignore_eos_rows[b]);
-    const bool eos = (id == st.eos_id) && !ignore;
+    // check_stop returns early while the slot holds fewer than min_tokens outputs (min_tokens <= max_new)
+    const int min_tok = ss.min_tokens != nullptr ? ss.min_tokens[b] : 0;
+    const bool core = n + 1 >= min_tok;
+    const bool eos = core && (id == st.eos_id) && !ignore;
     // vLLM's check_stop order: the primary eos, then the slot's stop set, then the length cap, so a stop id drawn as
     // the last allowed token reports "stop"
     bool stop = eos;
     int reason = -1;
-    if (!eos && st.stop_ids != nullptr) {
+    if (core && !eos && st.stop_ids != nullptr) {
       const int32_t* row = st.stop_ids + (int64_t)b * st.stop_stride;
       const int m = min(st.n_stop[b], st.stop_stride);
       for (int j = 0; j < m; ++j) {
@@ -494,9 +538,13 @@ __global__ void advance_kernel(prl_engine_state st) {
         }
       }
     }
+    int match = -1;
+    if (ss.tok_bytes != nullptr) match = match_stop_strings(ss, b, id, stop, n + 1 > min_tok);
+    if (match >= 0) stop = true;  // OutputProcessor: a matched string makes it "stop", even over "length"
     if (stop || n + 1 >= st.max_new[b]) {
       st.finished[b] = stop ? 1 : 2;  // 1 = stop, 2 = length
-      if (st.stop_reason != nullptr) st.stop_reason[b] = reason;
+      if (st.stop_reason != nullptr) st.stop_reason[b] = match >= 0 ? -1 : reason;
+      if (ss.stop_str_match != nullptr) ss.stop_str_match[b] = match;
       st.active[b] = 0;
       st.seq_lens[b] = 0;            // the slot stops reading its KV
       st.positions[b] = 0;
@@ -505,6 +553,22 @@ __global__ void advance_kernel(prl_engine_state st) {
   }
   st.positions[b] = next;
   st.seq_lens[b] = next + 1;
+}
+
+// ---- min_tokens: -inf on the slot's stop ids while it holds fewer than min_tokens outputs ----------------------------
+// One warp per row; a few ids per row.  Runs after the head GEMM, before the sampler reads the row.
+__global__ void ban_min_tokens_kernel(float* __restrict__ logits, int B, int V, const int32_t* __restrict__ gen_count,
+                                      const int32_t* __restrict__ min_tokens, const int32_t* __restrict__ ban_ids,
+                                      int ban_stride, const int32_t* __restrict__ n_ban) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= B || gen_count[b] >= min_tokens[b]) return;
+  const int m = min(n_ban[b], ban_stride);
+  for (int j = threadIdx.x & 31; j < m; j += 32) {
+    const int id = ban_ids[(int64_t)b * ban_stride + j];
+    if (id >= 0 && id < V) logits[(int64_t)b * V + id] = -INFINITY;
+  }
 }
 
 }  // namespace
@@ -662,7 +726,8 @@ extern "C" int prl_tp_epoch(void* epoch, prl_stream_t st) {
   return PRL_OK;
 }
 
-extern "C" int prl_advance_state(const prl_engine_state* state, prl_stream_t st) {
+extern "C" int prl_advance_state_strings(const prl_engine_state* state, const prl_stop_strings* strings,
+                                         prl_stream_t st) {
   PRL_CHECK_ARG(state && state->B >= 1, "prl_advance_state: bad argument");
   PRL_CHECK_ARG(state->sampled && state->sampled_logprobs && state->tokens && state->positions && state->seq_lens &&
                     state->active && state->prompt_buf && state->prompt_len && state->out_ids &&
@@ -670,7 +735,31 @@ extern "C" int prl_advance_state(const prl_engine_state* state, prl_stream_t st)
                 "prl_advance_state: NULL field");
   PRL_CHECK_ARG(state->stop_ids == nullptr || (state->n_stop && state->stop_stride >= 1),
                 "prl_advance_state: stop_ids needs n_stop and stop_stride >= 1");
-  PRL_CUDA(launch_pdl(advance_kernel, dim3((state->B + 127) / 128), dim3(128), 0, (cudaStream_t)st, *state));
+  prl_stop_strings ss = {};
+  if (strings != nullptr) ss = *strings;
+  PRL_CHECK_ARG(ss.tok_bytes == nullptr ||
+                    (ss.tok_offsets && ss.tok_special && ss.vocab >= 1 && ss.stop_str && ss.stop_str_fail &&
+                     ss.stop_str_len && ss.n_stop_str && ss.stop_str_flags && ss.stop_str_state &&
+                     ss.max_stop_str >= 1 && ss.stop_str_stride >= 1 && ss.stop_str_stride <= 32767),
+                "prl_advance_state_strings: tok_bytes needs the token table, every stop-string field, max_stop_str >= 1 "
+                "and 1 <= stop_str_stride <= 32767");
+  PRL_CUDA(launch_pdl(advance_kernel, dim3((state->B + 127) / 128), dim3(128), 0, (cudaStream_t)st, *state, ss));
+  PRL_LAUNCH_CHECK();
+  return PRL_OK;
+}
+
+extern "C" int prl_advance_state(const prl_engine_state* state, prl_stream_t st) {
+  return prl_advance_state_strings(state, nullptr, st);
+}
+
+extern "C" int prl_ban_min_tokens(float* logits, int32_t B, int32_t V, const int32_t* gen_count,
+                                  const int32_t* min_tokens, const int32_t* ban_ids, int32_t ban_stride,
+                                  const int32_t* n_ban, prl_stream_t st) {
+  PRL_CHECK_ARG(logits && gen_count && min_tokens && ban_ids && n_ban, "prl_ban_min_tokens: NULL argument");
+  PRL_CHECK_ARG(B >= 1 && V >= 1 && ban_stride >= 1, "prl_ban_min_tokens: bad shape (B=%d, V=%d, ban_stride=%d)", B, V,
+                ban_stride);
+  PRL_CUDA(launch_pdl(ban_min_tokens_kernel, dim3((B + 3) / 4), dim3(128), 0, (cudaStream_t)st, logits, (int)B, (int)V,
+                      gen_count, min_tokens, ban_ids, (int)ban_stride, n_ban));
   PRL_LAUNCH_CHECK();
   return PRL_OK;
 }

@@ -35,6 +35,10 @@ class SamplingParams:
     top_k: int = -1          # -1 / 0: off; 1 <= k < vocabulary: keep the k largest logits (and every tie of the k-th)
     top_p: float = 1.0       # 1: off; else keep the smallest top set holding mass >= top_p (vLLM's rule)
     stop_token_ids: tuple[int, ...] = ()   # ids that end the request with finish_reason "stop", even with ignore_eos
+    stop: tuple[str, ...] = ()             # stop strings (vLLM's `stop`); the output text is cut at the first match
+    min_tokens: int = 0                    # no stop (eos, stop ids, strings) before this many outputs; eos / stop ids banned
+    include_stop_str_in_output: bool = False   # vLLM's defaults; with stop strings only the pairs (True, False) and
+    skip_special_tokens: bool = True           # (False, True) are implemented
 
 
 def truncation_params(params: dict, greedy: bool = False) -> tuple[int, float]:
@@ -77,6 +81,127 @@ def stop_ids_from_generation_config(gen_cfg: dict, eos_token_id: int | None) -> 
     return (-1 if eos_token_id is None else int(eos_token_id)), tuple(sorted(int(i) for i in ids))
 
 
+def stop_strings_param(params: dict) -> tuple[str, ...]:
+    """`stop` of a request body / `llm.parameters`, validated as vLLM validates it (a string or a list of strings, none
+    empty; a missing or None value is empty).  Raises ValueError."""
+    stop = params.get("stop")
+    if stop is None:
+        return ()
+    if isinstance(stop, str):
+        stop = [stop]
+    if not isinstance(stop, (list, tuple)) or any(not isinstance(s, str) for s in stop):
+        raise ValueError(f"stop must be a string or a list of strings, got {stop!r}")
+    if any(s == "" for s in stop):
+        raise ValueError("stop cannot contain an empty string")
+    return tuple(stop)
+
+
+def min_tokens_param(params: dict, max_tokens: int) -> int:
+    """`min_tokens` of a request body / `llm.parameters`, validated as vLLM's SamplingParams._verify_args does
+    (0 <= min_tokens <= max_tokens; missing or None is 0).  Raises ValueError."""
+    m = params.get("min_tokens")
+    if m is None:
+        return 0
+    if isinstance(m, bool) or not isinstance(m, int):
+        raise ValueError(f"min_tokens must be an integer, got {m!r}")
+    if m < 0:
+        raise ValueError(f"min_tokens must be greater than or equal to 0, got {m}")
+    if m > max_tokens:
+        raise ValueError(f"min_tokens must be less than or equal to max_tokens={max_tokens}, got {m}")
+    return m
+
+
+def check_stop_flags(stop: tuple[str, ...], include_stop_str_in_output: bool, skip_special_tokens: bool) -> None:
+    """With stop strings, only the two flag pairs the reference's client sends are implemented: (True, False) when it
+    collects logprobs, vLLM's defaults (False, True) otherwise.  Raises ValueError for a mixed pair."""
+    if stop and bool(include_stop_str_in_output) == bool(skip_special_tokens):
+        raise ValueError("stop strings need include_stop_str_in_output and skip_special_tokens to be (true, false) or "
+                         f"(false, true); got ({bool(include_stop_str_in_output)}, {bool(skip_special_tokens)})")
+
+
+def _byte_decoder() -> dict[str, int]:
+    """Inverse of GPT-2's bytes_to_unicode: the printable character byte-level BPE writes for each byte."""
+    bs = list(range(ord("!"), ord("~") + 1)) + list(range(ord("\xa1"), ord("\xac") + 1)) + \
+        list(range(ord("\xae"), ord("\xff") + 1))
+    cs = bs[:]
+    n = 0
+    for b in range(256):
+        if b not in bs:
+            bs.append(b)
+            cs.append(256 + n)
+            n += 1
+    return {chr(c): b for b, c in zip(bs, cs)}
+
+
+def token_byte_table(tokenizer, vocab_size: int | None = None):
+    """(bytes uint8 [N], offsets int32 [V + 1], special uint8 [V]) of a byte-level BPE tokenizer (Qwen2, Qwen3, Llama 3):
+    an ordinary token's bytes are the byte-level decoding of its string, an added token's are its content, flagged when
+    it is special.  V is max(vocab_size, the tokenizer's size); ids the tokenizer does not have get no bytes.  Raises
+    ValueError for a tokenizer whose decoding is not the concatenation of per-token bytes, so that stop strings are
+    refused rather than matched against other text."""
+    import json
+
+    import numpy as np
+    backend = getattr(tokenizer, "backend_tokenizer", None) or getattr(tokenizer, "_tokenizer", None)
+    if backend is None or not hasattr(backend, "to_str"):
+        raise ValueError("stop strings need a fast (tokenizers) byte-level BPE tokenizer")
+    spec = json.loads(backend.to_str())
+    decoder, model = spec.get("decoder") or {}, spec.get("model") or {}
+    if decoder.get("type") != "ByteLevel" or model.get("type") != "BPE":
+        raise ValueError(f"stop strings need a byte-level BPE tokenizer (decoder {decoder.get('type')!r}, model "
+                         f"{model.get('type')!r}): its decoding is not a concatenation of per-token bytes")
+    added = {int(t["id"]): t for t in spec.get("added_tokens") or []}
+    vocab = {int(i): s for s, i in (model.get("vocab") or {}).items()}
+    n_ids = max([-1, *vocab, *added]) + 1
+    V = max(n_ids, int(vocab_size or 0))
+    inv = _byte_decoder()
+    chunks, offsets, special = [], np.zeros(V + 1, dtype=np.int32), np.zeros(V, dtype=np.uint8)
+    at = 0
+    for t in range(V):
+        if t in added:
+            b = added[t]["content"].encode("utf-8")
+            special[t] = int(bool(added[t].get("special")))
+        elif t in vocab:
+            try:
+                b = bytes(inv[c] for c in vocab[t])
+            except KeyError as e:
+                raise ValueError(f"token {t} ({vocab[t]!r}) is not byte-level encoded") from e
+        else:
+            b = b""
+        chunks.append(b)
+        at += len(b)
+        offsets[t + 1] = at
+    data = np.frombuffer(b"".join(chunks) or b"\0", dtype=np.uint8).copy()
+    return data, offsets, special
+
+
+def kmp_failure(s: bytes) -> list[int]:
+    """fail[i] = length of the longest proper prefix of s[:i + 1] that is also its suffix (the matcher's fallback)."""
+    fail, k = [0] * len(s), 0
+    for i in range(1, len(s)):
+        while k > 0 and s[i] != s[k]:
+            k = fail[k - 1]
+        if s[i] == s[k]:
+            k += 1
+        fail[i] = k
+    return fail
+
+
+def utf8_text(data: bytes) -> str:
+    """What an incremental detokenizer has emitted after `data`: complete characters only (a trailing incomplete UTF-8
+    sequence is held back), invalid bytes as U+FFFD."""
+    cut = len(data)
+    for k in range(1, min(4, len(data)) + 1):
+        c = data[-k]
+        if c & 0xC0 == 0x80:
+            continue
+        need = 2 if c & 0xE0 == 0xC0 else 3 if c & 0xF0 == 0xE0 else 4 if c & 0xF8 == 0xF0 else 1
+        if need > k:
+            cut = len(data) - k
+        break
+    return data[:cut].decode("utf-8", errors="replace")
+
+
 def requested_truncation(top_k: int, top_p: float) -> set[str]:
     """The truncation features a validated (top_k, top_p) pair asks for."""
     return ({"top_k"} if top_k > 0 else set()) | ({"top_p"} if top_p < 1.0 else set())
@@ -92,7 +217,9 @@ class Request:
     output_ids: list[int] = field(default_factory=list)
     output_logprobs: list[float] = field(default_factory=list)
     finish_reason: str | None = None
-    stop_reason: int | None = None                       # the stop id that ended it (vLLM's stop_reason); None for eos / length
+    stop_reason: int | str | None = None                 # the stop id or stop string that ended it (vLLM's stop_reason);
+                                                         # None for eos / length
+    output_text: str | None = None                       # vLLM's output_text, for requests with stop strings
     model_version: int = 0
     prefilled: int = 0                                   # prompt tokens whose KV is in the cache
     waits_for: list = field(default_factory=list)        # [(request filling a shared page, tokens it must reach)]
@@ -102,7 +229,8 @@ class DecodeEngine:
     def __init__(self, cfg: ModelConfig, arena: ParamArena, max_batch: int = 64, max_seq_len: int = 16384,
                  n_pages: int | None = None, max_new_tokens: int = 8192, eos_id: int = -1, seed: int = 42,
                  device: torch.device | str = "cuda:0", use_cuda_graph: bool = True, prefill_chunk: int = 1024,
-                 prefix_sharing: bool = True, fused_head: bool = False, stop_ids=(), max_stop_ids: int = 16):
+                 prefix_sharing: bool = True, fused_head: bool = False, stop_ids=(), max_stop_ids: int = 16,
+                 tokenizer=None, max_stop_strings: int = 8, max_stop_str_bytes: int = 64):
         if cfg.head_dim != 128:
             raise ValueError("the sm_90a attention kernel is built for head_dim 128")
         self.cfg, self.arena = cfg, arena
@@ -190,6 +318,30 @@ class DecodeEngine:
         self.n_stop = torch.zeros(B, dtype=torch.int32, device=d)
         self.stop_reason = torch.full((B,), -1, dtype=torch.int32, device=d)
         self._stop_slots: set[int] = set()
+        # stop strings (tokenizer given) and min_tokens per slot; like the stop sets, the advance kernel gets their fields
+        # and the ban kernel runs only while some slot uses them, so without them the step is what it was before
+        self.max_stop_strings, self.max_stop_str_bytes = int(max_stop_strings), int(max_stop_str_bytes)
+        if not (1 <= self.max_stop_strings and 1 <= self.max_stop_str_bytes <= 32767):
+            raise ValueError("max_stop_strings must be >= 1 and max_stop_str_bytes in [1, 32767]")
+        self._tok_table = None
+        if tokenizer is not None:
+            data, offsets, special = token_byte_table(tokenizer, cfg.vocab_size)
+            self._tok_table = (torch.from_numpy(data).to(d), torch.from_numpy(offsets).to(d),
+                               torch.from_numpy(special).to(d), len(special))
+        S, L = self.max_stop_strings, self.max_stop_str_bytes
+        self.stop_str = torch.zeros(B, S, L, dtype=torch.uint8, device=d)
+        self.stop_str_fail = torch.zeros(B, S, L, dtype=torch.int16, device=d)
+        self.stop_str_len = torch.ones(B, S, **i32)
+        self.n_stop_str = torch.zeros(B, **i32)
+        self.stop_str_flags = torch.zeros(B, dtype=torch.uint8, device=d)
+        self.stop_str_state = torch.zeros(B, S, **i32)
+        self.stop_str_match = torch.full((B,), -1, **i32)
+        self._str_slots: set[int] = set()
+        self.min_tokens_rows = torch.zeros(B, **i32)
+        self.ban_stride = 1 + len(self.stop_ids) + self.max_stop_ids
+        self.ban_rows = torch.zeros(B, self.ban_stride, **i32)
+        self.n_ban = torch.zeros(B, **i32)
+        self._min_slots: set[int] = set()
         self._temperature, self._greedy, self._ignore_eos = 1.0, False, False
         self._graphs: dict[int, torch.cuda.CUDAGraph] = {}
         # ---- chunked prefill + prefix sharing (GRPO attempts share their prompt) ----
@@ -218,6 +370,16 @@ class DecodeEngine:
     # per-request stop_token_ids: the state advance checks each slot's stop set, so every engine that calls
     # prl_advance_state (fused head and TP included) has them; clients read this before sending stop ids
     supports_stop_token_ids = True
+
+    @property
+    def supports_stop_strings(self) -> bool:
+        """Stop strings are matched in the state advance (both head paths) once a token byte table is installed."""
+        return self._tok_table is not None
+
+    @property
+    def supports_min_tokens(self) -> bool:
+        """The min_tokens ban writes -inf into the logits, which only the unfused head keeps in HBM."""
+        return not self.fused_head
 
     # engine-wide sampling defaults: assigning one overwrites every slot (benches, tools, single-tenant tests)
     @property
@@ -272,13 +434,36 @@ class DecodeEngine:
         s.eos_id, s.ignore_eos = self.eos_id, 0
         s.ignore_eos_rows = self.ignore_eos_rows.data_ptr()
         s.stop_stride, s.n_stop = self.max_stop_ids, self.n_stop.data_ptr()
+        x = self._strings = _lib.StopStrings()
+        if self._tok_table is not None:
+            _, to, ts, x.vocab = self._tok_table
+            x.tok_offsets, x.tok_special = to.data_ptr(), ts.data_ptr()
+        x.stop_str, x.stop_str_fail = self.stop_str.data_ptr(), self.stop_str_fail.data_ptr()
+        x.stop_str_len, x.n_stop_str = self.stop_str_len.data_ptr(), self.n_stop_str.data_ptr()
+        x.max_stop_str, x.stop_str_stride = self.max_stop_strings, self.max_stop_str_bytes
+        x.stop_str_flags, x.stop_str_state = self.stop_str_flags.data_ptr(), self.stop_str_state.data_ptr()
+        x.stop_str_match = self.stop_str_match.data_ptr()
         return s
 
     def _advance(self, st: int) -> None:
         on = bool(self._stop_slots)
         self._state.stop_ids = self.stop_rows.data_ptr() if on else None
         self._state.stop_reason = self.stop_reason.data_ptr() if on else None
-        _lib.check(self.lib.prl_advance_state(C.byref(self._state), st))
+        if not (self._str_slots or self._min_slots):
+            _lib.check(self.lib.prl_advance_state(C.byref(self._state), st))
+            return
+        # tok_bytes switches the string matcher on; the other string fields are set once in _make_state
+        self._strings.tok_bytes = self._tok_table[0].data_ptr() if self._str_slots else None
+        self._strings.min_tokens = self.min_tokens_rows.data_ptr() if self._min_slots else None
+        _lib.check(self.lib.prl_advance_state_strings(C.byref(self._state), C.byref(self._strings), st))
+
+    def _ban_min_tokens(self, st: int) -> None:
+        """-inf on each min_tokens slot's stop ids (eos, generation_config's and its own) while it is short of
+        min_tokens outputs: vLLM's MinTokensLogitsProcessor, between the head GEMM and the sampler."""
+        if self._min_slots:
+            _lib.check(self.lib.prl_ban_min_tokens(self.logits.data_ptr(), self.B, self.cfg.head_rows,
+                                                   self.gen_count.data_ptr(), self.min_tokens_rows.data_ptr(),
+                                                   self.ban_rows.data_ptr(), self.ban_stride, self.n_ban.data_ptr(), st))
 
     # ------------------------------------------------------------------------------------------
     def _gemm(self, w_name: str, x: torch.Tensor, n: int, k: int, split: int, out: torch.Tensor, lo: str | None = None,
@@ -379,6 +564,7 @@ class DecodeEngine:
                                             self.head_ws.data_ptr(), self.head_ws.numel(), st))
             self._advance(st)
             return
+        self._ban_min_tokens(st)
         if self._truncated_slots:
             _lib.check(lib.prl_sample_logprob_topkp_rows(self.logits.data_ptr(), self.B, self.cfg.head_rows,
                                                          self.inv_temp_rows.data_ptr(), self.greedy_rows.data_ptr(),
@@ -463,6 +649,63 @@ class DecodeEngine:
         if len(row) > self.max_stop_ids:
             raise ValueError(f"{len(row)} stop token ids exceed this engine's limit of {self.max_stop_ids}")
         return row
+
+    def stop_string_rows(self, params: SamplingParams) -> list[bytes]:
+        """The UTF-8 bytes of a request's stop strings, one matcher row each.  Raises ValueError when the engine has no
+        token byte table, for a flag pair other than the two implemented, or past the rows' limits."""
+        stop = stop_strings_param({"stop": list(params.stop) if params.stop else None})
+        if not stop:
+            return []
+        if not self.supports_stop_strings:
+            raise ValueError(f"stop strings are not implemented by this engine ({type(self).__name__}: "
+                             "build it with a byte-level tokenizer)")
+        check_stop_flags(stop, params.include_stop_str_in_output, params.skip_special_tokens)
+        if len(stop) > self.max_stop_strings:
+            raise ValueError(f"{len(stop)} stop strings exceed this engine's limit of max_stop_strings="
+                             f"{self.max_stop_strings}")
+        rows = [s.encode("utf-8") for s in stop]
+        for s, b in zip(stop, rows):
+            if len(b) > self.max_stop_str_bytes:
+                raise ValueError(f"stop string {s!r} has {len(b)} bytes, over this engine's limit of "
+                                 f"max_stop_str_bytes={self.max_stop_str_bytes}")
+        return rows
+
+    def min_tokens_ban_row(self, params: SamplingParams) -> list[int]:
+        """vLLM's SamplingParams.all_stop_token_ids: the primary eos, generation_config's other eos ids and the request's
+        stop_token_ids, whatever ignore_eos says."""
+        ids = ([self.eos_id] if self.eos_id >= 0 else []) + list(self.stop_ids) + list(params.stop_token_ids)
+        return list(dict.fromkeys(ids))
+
+    def stop_string_text(self, req: Request, match: int) -> str:
+        """vLLM's output_text of a finished request with stop strings (IncrementalDetokenizer.update): the text of its
+        tokens under the request's flags, cut at the stop string `match` (an index into params.stop, -1: none) found in
+        the text the last token added."""
+        p = req.params
+        data, offsets, special, V = self._tok_table_host()
+        ids = list(req.output_ids)
+        fed = ids
+        if match < 0 and req.finish_reason == "stop" and not p.include_stop_str_in_output:
+            fed = ids[:-1]                 # the eos / stop id that ended it is not detokenized
+
+        def text_of(seq):
+            out = bytearray()
+            for t in seq:
+                if 0 <= t < V and not (p.skip_special_tokens and special[t]):
+                    out += data[offsets[t]:offsets[t + 1]]
+            return utf8_text(bytes(out))
+        text = text_of(fed)
+        if match < 0:
+            return text
+        stop = p.stop[match]
+        new = len(text) - len(text_of(fed[:-1]))
+        at = text.find(stop, max(0, len(text) + 1 - new - len(stop)))
+        return text[:at + len(stop)] if p.include_stop_str_in_output else text[:at]
+
+    def _tok_table_host(self):
+        if not hasattr(self, "_tok_host"):
+            data, offsets, special, V = self._tok_table
+            self._tok_host = (data.cpu().numpy().tobytes(), offsets.cpu().tolist(), special.cpu().tolist(), V)
+        return self._tok_host
 
     # ---- chunked prefill ------------------------------------------------------------------------
     def _prefill_buffers(self):
@@ -693,6 +936,11 @@ class DecodeEngine:
             raise ValueError(f"{' / '.join(sorted(missing))} sampling is not implemented by this engine "
                              f"({type(self).__name__}, fused_head={self.fused_head})")
         stop = self.stop_row(params)
+        strings = self.stop_string_rows(params)
+        min_tokens = min_tokens_param({"min_tokens": params.min_tokens}, params.max_tokens)
+        if min_tokens and not self.supports_min_tokens:
+            raise ValueError(f"min_tokens is not implemented by this engine ({type(self).__name__}, "
+                             f"fused_head={self.fused_head})")
         if not self.can_admit(n, params.max_tokens):
             raise RuntimeError("engine full")
         req = Request(self._next_id, list(prompt_ids), params, model_version=model_version)
@@ -754,6 +1002,28 @@ class DecodeEngine:
             self.n_stop[slot] = len(stop)
             self.stop_rows[slot, :len(stop)].copy_(torch.tensor(stop, dtype=torch.int32), non_blocking=True)
             self._stop_slots.add(slot)
+        if strings:
+            S, L = self.max_stop_strings, self.max_stop_str_bytes
+            rows, fails, lens = torch.zeros(S, L, dtype=torch.uint8), torch.zeros(S, L, dtype=torch.int16), torch.ones(S, dtype=torch.int32)
+            for j, b in enumerate(strings):
+                rows[j, :len(b)] = torch.tensor(list(b), dtype=torch.uint8)
+                fails[j, :len(b)] = torch.tensor(kmp_failure(b), dtype=torch.int16)
+                lens[j] = len(b)
+            self.stop_str[slot].copy_(rows, non_blocking=True)
+            self.stop_str_fail[slot].copy_(fails, non_blocking=True)
+            self.stop_str_len[slot].copy_(lens, non_blocking=True)
+            self.n_stop_str[slot] = len(strings)
+            self.stop_str_flags[slot] = int(bool(params.include_stop_str_in_output)) | 2 * int(bool(params.skip_special_tokens))
+            self.stop_str_state[slot].zero_()
+            self.stop_str_match[slot] = -1
+            self._str_slots.add(slot)
+        if min_tokens:
+            ban = self.min_tokens_ban_row(params)
+            self.min_tokens_rows[slot] = min_tokens
+            self.n_ban[slot] = len(ban)
+            if ban:
+                self.ban_rows[slot, :len(ban)].copy_(torch.tensor(ban, dtype=torch.int32), non_blocking=True)
+            self._min_slots.add(slot)
         self.tokens[slot] = prompt_ids[start]
         self.positions[slot] = start
         self.seq_lens[slot] = start + 1
@@ -782,6 +1052,16 @@ class DecodeEngine:
                 self._stop_slots.discard(slot)
                 self.n_stop[slot] = 0
                 req.stop_reason = int(reason[slot]) if code == 1 and int(reason[slot]) >= 0 else None
+            if slot in self._str_slots:
+                self._str_slots.discard(slot)
+                self.n_stop_str[slot] = 0
+                match = int(self.stop_str_match[slot].item()) if code == 1 else -1
+                if match >= 0:
+                    req.stop_reason = req.params.stop[match]
+                req.output_text = self.stop_string_text(req, match)
+            if slot in self._min_slots:
+                self._min_slots.discard(slot)
+                self.min_tokens_rows[slot] = 0
             self.block_table[slot].zero_()
             self.finished[slot] = 0
             if slot in self._truncated_slots:

@@ -35,7 +35,8 @@ from typing import Any
 
 from aiohttp import web
 
-from .engine import SamplingParams, requested_truncation, stop_token_ids_param, truncation_params
+from .engine import (SamplingParams, check_stop_flags, min_tokens_param, requested_truncation, stop_strings_param,
+                     stop_token_ids_param, truncation_params)
 from .serving import engine_features
 
 
@@ -110,9 +111,15 @@ class HttpShim:
 
     def _sampling(self, body: dict) -> SamplingParams | web.Response:
         temperature = float(body.get("temperature", 1.0))
+        max_tokens = int(body.get("max_tokens") or body.get("max_completion_tokens") or self.default_max_tokens)
+        include = bool(body.get("include_stop_str_in_output", False))
+        skip = bool(body.get("skip_special_tokens", True))
         try:
             top_k, top_p = truncation_params(body, greedy=temperature <= 0)
             stop_ids = stop_token_ids_param(body)
+            stop = stop_strings_param(body)
+            min_tokens = min_tokens_param(body, max_tokens)
+            check_stop_flags(stop, include, skip)
         except ValueError as e:
             return self._bad(str(e))
         engine = getattr(self.server, "engine", None)
@@ -122,16 +129,22 @@ class HttpShim:
             return self._bad(f"{' / '.join(sorted(missing))} sampling is not implemented by this engine")
         if stop_ids and "stop_token_ids" not in features:
             return self._bad("stop_token_ids are not implemented by this engine")
+        if stop and "stop" not in features:
+            return self._bad("stop strings are not implemented by this engine")
+        if min_tokens and "min_tokens" not in features:
+            return self._bad("min_tokens is not implemented by this engine")
         if int(body.get("n", 1)) != 1 or body.get("stream"):
             return self._bad("n > 1 and streaming are not implemented")
-        max_tokens = int(body.get("max_tokens") or body.get("max_completion_tokens") or self.default_max_tokens)
         sp = SamplingParams(max_tokens=max_tokens, temperature=temperature if temperature > 0 else 1.0,
-                            greedy=temperature <= 0, top_k=top_k, top_p=top_p, stop_token_ids=stop_ids)
-        if stop_ids:
-            try:
+                            greedy=temperature <= 0, top_k=top_k, top_p=top_p, stop_token_ids=stop_ids, stop=stop,
+                            min_tokens=min_tokens, include_stop_str_in_output=include, skip_special_tokens=skip)
+        try:
+            if stop_ids:
                 engine.stop_row(sp)        # ids outside the vocabulary, or more than a slot's stop row holds
-            except ValueError as e:
-                return self._bad(str(e))
+            if stop:
+                engine.stop_string_rows(sp)   # more strings or longer ones than a slot's rows hold
+        except ValueError as e:
+            return self._bad(str(e))
         return sp
 
     async def chat_completions(self, request: web.Request) -> web.Response:
@@ -148,8 +161,9 @@ class HttpShim:
         prompt_ids = _token_ids(self.tok.apply_chat_template(messages, add_generation_prompt=True, **kw))
         req = await self.server.generate(prompt_ids, sp)
         out_ids = list(req.output_ids)
-        # include_stop_str_in_output / skip_special_tokens=False (what the reference asks for): decode every id
-        content = self._decode(out_ids)
+        # include_stop_str_in_output / skip_special_tokens=False (what the reference asks for): decode every id; with
+        # stop strings the content is vLLM's output_text, which the engine computed under the request's flags
+        content = req.output_text if sp.stop and getattr(req, "output_text", None) is not None else self._decode(out_ids)
         choice: dict[str, Any] = {"index": 0, "message": {"role": "assistant", "content": content, "tool_calls": []},
                                   "finish_reason": req.finish_reason, "stop_reason": getattr(req, "stop_reason", None)}
         if body.get("logprobs"):

@@ -39,9 +39,11 @@ def sampling_features(base_url: str) -> frozenset:
 
 
 def engine_features(engine) -> frozenset:
-    """An engine's `sampling_features`, plus "stop_token_ids" when it sets `supports_stop_token_ids`."""
-    stop = {"stop_token_ids"} if getattr(engine, "supports_stop_token_ids", False) else set()
-    return frozenset(getattr(engine, "sampling_features", frozenset())) | stop
+    """An engine's `sampling_features`, plus "stop_token_ids" when it sets `supports_stop_token_ids`, "stop" (stop
+    strings) when it sets `supports_stop_strings` and "min_tokens" when it sets `supports_min_tokens`."""
+    extra = {name for name, attr in (("stop_token_ids", "supports_stop_token_ids"), ("stop", "supports_stop_strings"),
+                                     ("min_tokens", "supports_min_tokens")) if getattr(engine, attr, False)}
+    return frozenset(getattr(engine, "sampling_features", frozenset())) | extra
 
 
 @dataclass

@@ -30,6 +30,9 @@ class TPDecodeEngine(DecodeEngine):
     # the vocab-parallel head exchanges 16 sampler partials per row, not logits: no rank sees the whole row that a
     # top-k / top-p threshold is taken over, so add_request refuses truncation here
     sampling_features = frozenset()
+    # neither stop strings nor min_tokens: add_request refuses both here
+    supports_stop_strings = False
+    supports_min_tokens = False
 
     def __init__(self, full_cfg: ModelConfig, arena: ParamArena, tp_rank: int, tp_size: int, group=None, **kw):
         import torch.distributed as dist
