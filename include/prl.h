@@ -599,6 +599,38 @@ int prl_ban_min_tokens(float* logits /*[B,V]*/, int32_t B, int32_t V, const int3
                        const int32_t* ban_ids /*[B, ban_stride]*/, int32_t ban_stride, const int32_t* n_ban,
                        prl_stream_t stream);
 
+/* Repetition / frequency / presence penalties and min_p (vLLM's apply_penalties and MinPLogitsProcessor), in place on
+ * the logits between the min_tokens ban and the sampler.  One CTA per row; a row with presence 0, frequency 0,
+ * repetition 1 and min_p 0 (or greedy) is not touched.  For a row with a non-default penalty:
+ *   - seen[b] < 0 (a new request): its count row is zeroed and its prompt mask rebuilt from prompt_buf[b, :prompt_len];
+ *   - out_ids[b, seen:gen_count] are added to its count row and seen[b] = gen_count[b], so the counts are those of the
+ *     outputs before this step;
+ *   - each logit l, in this order, each step one fp32 rounding:  masked by prompt | output:  l = l > 0 ? l * (1/r) : l * r;
+ *     l -= f * count;  l -= pr * (count > 0).
+ * Then, for a row with min_p > 0 that is not greedy: with z = l * inv_temp and m = max z, l = -inf where
+ * exp(z - m) < min_p.  Ids outside [0, V) in the prompt or outputs are skipped. */
+typedef struct {
+  float* logits;                   /* [B, V] in/out */
+  int32_t B;
+  int32_t V;
+  const float* presence;           /* [B] */
+  const float* frequency;          /* [B] */
+  const float* repetition;         /* [B] > 0 */
+  const float* min_p;              /* [B] in [0, 1] */
+  const float* inv_temp;           /* [B] the samplers' 1 / temperature rows */
+  const uint8_t* greedy;           /* [B] */
+  const int32_t* prompt_buf;       /* [B, prompt_stride] */
+  int32_t prompt_stride;
+  const int32_t* prompt_len;       /* [B] */
+  const int32_t* out_ids;          /* [B, out_stride] */
+  int32_t out_stride;
+  const int32_t* gen_count;        /* [B] */
+  int32_t* counts;                 /* [B, V] output counts per id */
+  uint32_t* prompt_mask;           /* [B, (V + 31) / 32] bit id: the id is in the prompt */
+  int32_t* seen;                   /* [B] outputs already in counts; -1: reset the row */
+} prl_penalties;
+int prl_apply_penalties(const prl_penalties* p, prl_stream_t stream);
+
 /* ---- tensor parallelism inside one engine (BASELINE config 4: Qwen2.5-32B, TP=2; the reference passes
  * tensor-parallel-size to vLLM, world.py:56-59, which all-reduces twice per layer with NCCL/custom all-reduce).
  * Here the row-parallel GEMMs (o_proj, down_proj) store their fp32 partial tiles into the local AND the peer GPU's

@@ -89,6 +89,16 @@ class StopStrings(C.Structure):
     ]
 
 
+class Penalties(C.Structure):
+    _fields_ = [
+        ("logits", C.c_void_p), ("B", C.c_int32), ("V", C.c_int32), ("presence", C.c_void_p), ("frequency", C.c_void_p),
+        ("repetition", C.c_void_p), ("min_p", C.c_void_p), ("inv_temp", C.c_void_p), ("greedy", C.c_void_p),
+        ("prompt_buf", C.c_void_p), ("prompt_stride", C.c_int32), ("prompt_len", C.c_void_p), ("out_ids", C.c_void_p),
+        ("out_stride", C.c_int32), ("gen_count", C.c_void_p), ("counts", C.c_void_p), ("prompt_mask", C.c_void_p),
+        ("seen", C.c_void_p),
+    ]
+
+
 class MbRecord(C.Structure):
     _fields_ = [("n_chunk", C.c_int32), ("n_pack", C.c_int32), ("padding", C.c_int32), ("total_tok", C.c_int32),
                 ("total_lp", C.c_int32), ("n_stat_slots", C.c_int32), ("n_rollout_slots", C.c_int32), ("n_groups", C.c_int32),
@@ -235,6 +245,7 @@ _SIGNATURES = {
     "prl_advance_state_strings": (C.c_int, [C.POINTER(EngineState), C.POINTER(StopStrings), C.c_void_p]),
     "prl_ban_min_tokens": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                      C.c_void_p, C.c_void_p]),
+    "prl_apply_penalties": (C.c_int, [C.POINTER(Penalties), C.c_void_p]),
     "prl_gemm_bf16_splitk_peer": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
                                             C.c_void_p, C.c_void_p, C.c_void_p]),
     "prl_tp_signal": (C.c_int, [C.c_void_p, C.c_void_p]),

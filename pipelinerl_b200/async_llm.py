@@ -2,8 +2,8 @@
 (reference: pipelinerl/async_llm.py:86-212 and :215-346)."""
 from __future__ import annotations
 
-from .engine import (SamplingParams, check_stop_flags, min_tokens_param, requested_truncation, stop_strings_param,
-                     stop_token_ids_param, truncation_params)
+from .engine import (SamplingParams, check_stop_flags, min_tokens_param, penalty_params, requested_penalties,
+                     requested_truncation, stop_strings_param, stop_token_ids_param, truncation_params)
 from .llm import LLMCall, LLMOutput, Prompt, TokenLogprob, TrainableLLM
 from .rollouts import TrainingText, apply_rollout_reward
 from .serving import resolve, sampling_features
@@ -35,14 +35,17 @@ def _chat_kwargs(llm: TrainableLLM, prompt: Prompt) -> dict:
     return kw
 
 
-def _reject_unsupported_sampling(params: dict, features: frozenset = frozenset()) -> tuple[int, float, tuple[int, ...]]:
+def _reject_unsupported_sampling(params: dict, features: frozenset = frozenset()
+                                 ) -> tuple[int, float, tuple[int, ...], tuple[float, float, float, float]]:
     """Sampling features the engine does not implement must fail loudly, exactly as http_shim.py answers 400 for them:
     a silently ignored top_p / top_k / stop would make the recorded logprobs those of a different distribution than the
     one the request asked for.  top_k / top_p are accepted when the target engine lists them in `features` (the unfused
     single-GPU DecodeEngine does; the reference's eval handles send top_p 0.95 / top_k 50, conf/base.yaml:52-57), and
     stop_token_ids when it lists "stop_token_ids"; they are validated as vLLM validates them.  Stop strings and
-    min_tokens > 0 are refused unless it lists "stop" / "min_tokens" (stop_params validates them).
-    Returns the request's (top_k, top_p, stop_token_ids)."""
+    min_tokens > 0 are refused unless it lists "stop" / "min_tokens" (stop_params validates them), and
+    presence_penalty, frequency_penalty, repetition_penalty and min_p away from their defaults unless it lists each of
+    them (validated as vLLM validates them).
+    Returns the request's (top_k, top_p, stop_token_ids, (presence, frequency, repetition, min_p))."""
     greedy = float(params.get("temperature", 1.0)) <= 0
     top_k, top_p = truncation_params(params, greedy=greedy)
     missing = requested_truncation(top_k, top_p) - features
@@ -55,10 +58,11 @@ def _reject_unsupported_sampling(params: dict, features: frozenset = frozenset()
         raise ValueError("stop strings are not implemented by this engine (stop token ids are)")
     if int(params.get("n", 1)) != 1:
         raise ValueError("n > 1 completions per request is not implemented (the actor issues `attempts` requests)")
-    for name in ("presence_penalty", "frequency_penalty", "repetition_penalty", "min_p"):
-        if params.get(name) not in (None, 0, 0.0, 1, 1.0) or (name == "repetition_penalty" and params.get(name) not in (None, 1, 1.0)):
-            raise ValueError(f"sampling parameter {name} is not implemented by this engine")
-    return top_k, top_p, stop_ids
+    penalties = penalty_params(params, greedy=greedy)
+    missing = requested_penalties(penalties) - features
+    if missing:
+        raise ValueError(f"sampling parameter {' / '.join(sorted(missing))} is not implemented by this engine")
+    return top_k, top_p, stop_ids, penalties
 
 
 def stop_params(params: dict, features: frozenset, max_tokens: int,
@@ -90,7 +94,7 @@ async def llm_async_generate(llm: TrainableLLM, prompt: Prompt, session=None,
                                                                         **_chat_kwargs(llm, prompt)))
     params = llm.parameters
     features = sampling_features(llm.base_url)
-    top_k, top_p, stop_ids = _reject_unsupported_sampling(params, features)
+    top_k, top_p, stop_ids, penalties = _reject_unsupported_sampling(params, features)
     max_tokens = int(max_tokens_override if max_tokens_override is not None else params.get("max_tokens", 16))
     stop, min_tokens, include, skip = stop_params(params, features, max_tokens, bool(llm.collect_logprobs))
     temperature = float(params.get("temperature", 1.0))
@@ -98,6 +102,7 @@ async def llm_async_generate(llm: TrainableLLM, prompt: Prompt, session=None,
                         greedy=temperature <= 0, ignore_eos=bool(params.get("ignore_eos", False)), top_k=top_k,
                         top_p=top_p, stop_token_ids=stop_ids, stop=stop, min_tokens=min_tokens,
                         include_stop_str_in_output=include, skip_special_tokens=skip)
+    sp.presence_penalty, sp.frequency_penalty, sp.repetition_penalty, sp.min_p = penalties
     server = resolve(llm.base_url)
     if stop_ids:
         server.engine.stop_row(sp)      # out-of-vocabulary ids or too many: ValueError here, not on the engine thread

@@ -571,6 +571,112 @@ __global__ void ban_min_tokens_kernel(float* __restrict__ logits, int B, int V, 
   }
 }
 
+// ---- penalties and min_p: vLLM's apply_penalties, then MinPLogitsProcessor after the temperature ---------------------
+// One CTA per row; the row is streamed once for the penalties (logits, counts, prompt-mask words) and once more for
+// min_p.  Each penalty step is its own fp32 rounding, as vLLM's three tensor ops are (no FMA contraction).  Counts and
+// mask words are read through L2 (__ldcg): this CTA has just written them with plain stores and atomics.
+constexpr int kPenThreads = 1024;
+
+__device__ __forceinline__ float penalize(float l, int c, uint32_t prompt_word, int i, float r, float inv_r, float f,
+                                          float pr) {
+  if (c > 0 || ((prompt_word >> (i & 31)) & 1u)) l = __fmul_rn(l, l > 0.f ? inv_r : r);  // unmasked: vLLM's * 1.0
+  l = __fsub_rn(l, __fmul_rn(f, (float)c));
+  return __fsub_rn(l, __fmul_rn(pr, c > 0 ? 1.f : 0.f));
+}
+
+__device__ __forceinline__ float zmax4(float m, float4 l, float inv_temp) {
+  return fmaxf(fmaxf(m, fmaxf(__fmul_rn(l.x, inv_temp), __fmul_rn(l.y, inv_temp))),
+               fmaxf(__fmul_rn(l.z, inv_temp), __fmul_rn(l.w, inv_temp)));
+}
+
+__global__ void __launch_bounds__(kPenThreads) penalties_kernel(prl_penalties p) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x, V = p.V;
+  const float pr = p.presence[b], f = p.frequency[b], r = p.repetition[b];
+  const float min_p = p.greedy[b] ? 0.f : p.min_p[b];   // vLLM resets min_p for greedy requests
+  const bool pen = pr != 0.f || f != 0.f || r != 1.f;
+  const bool use_min_p = min_p > 0.f;
+  if (!pen && !use_min_p) return;
+  float* row = p.logits + (int64_t)b * V;
+  const float inv_temp = p.inv_temp[b];
+  // 16-byte rows: four ids per load, so that one CTA keeps enough bytes in flight to stream its row
+  const bool vec = (V & 3) == 0 && ((uintptr_t)p.logits & 15) == 0 && ((uintptr_t)p.counts & 15) == 0;
+  float4* row4 = reinterpret_cast<float4*>(row);
+  const int V4 = vec ? V >> 2 : 0;
+  float m = -INFINITY;
+  if (pen) {
+    int32_t* cnt = p.counts + (int64_t)b * V;
+    const int W = (V + 31) >> 5;
+    uint32_t* mask = p.prompt_mask + (int64_t)b * W;
+    int seen = p.seen[b];
+    const int n_out = min(p.gen_count[b], p.out_stride);
+    if (seen < 0) {                       // first launch for this request: fresh counts, its own prompt mask
+      for (int i = threadIdx.x; i < V; i += kPenThreads) cnt[i] = 0;
+      for (int i = threadIdx.x; i < W; i += kPenThreads) mask[i] = 0u;
+      __syncthreads();
+      const int32_t* prompt = p.prompt_buf + (int64_t)b * p.prompt_stride;
+      const int n_prompt = min(p.prompt_len[b], p.prompt_stride);
+      for (int i = threadIdx.x; i < n_prompt; i += kPenThreads) {
+        const int id = prompt[i];
+        if (id >= 0 && id < V) atomicOr(&mask[id >> 5], 1u << (id & 31));
+      }
+      seen = 0;
+    }
+    const int32_t* out = p.out_ids + (int64_t)b * p.out_stride;
+    for (int i = seen + threadIdx.x; i < n_out; i += kPenThreads) {
+      const int id = out[i];
+      if (id >= 0 && id < V) atomicAdd(&cnt[id], 1);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) p.seen[b] = max(seen, n_out);
+    const float inv_r = __fdiv_rn(1.f, r);
+    const int4* cnt4 = reinterpret_cast<const int4*>(cnt);
+#pragma unroll 2
+    for (int j = threadIdx.x; j < V4; j += kPenThreads) {
+      float4 l = row4[j];
+      const int4 c = __ldcg(cnt4 + j);
+      const uint32_t w = __ldcg(mask + (j >> 3));
+      const int i = j << 2;
+      l.x = penalize(l.x, c.x, w, i, r, inv_r, f, pr);
+      l.y = penalize(l.y, c.y, w, i + 1, r, inv_r, f, pr);
+      l.z = penalize(l.z, c.z, w, i + 2, r, inv_r, f, pr);
+      l.w = penalize(l.w, c.w, w, i + 3, r, inv_r, f, pr);
+      row4[j] = l;
+      m = zmax4(m, l, inv_temp);
+    }
+    for (int i = (V4 << 2) + threadIdx.x; i < V; i += kPenThreads) {
+      const float l = penalize(row[i], __ldcg(cnt + i), __ldcg(mask + (i >> 5)), i, r, inv_r, f, pr);
+      row[i] = l;
+      m = fmaxf(m, __fmul_rn(l, inv_temp));
+    }
+  } else {
+#pragma unroll 4
+    for (int j = threadIdx.x; j < V4; j += kPenThreads) m = zmax4(m, row4[j], inv_temp);
+    for (int i = (V4 << 2) + threadIdx.x; i < V; i += kPenThreads) m = fmaxf(m, __fmul_rn(row[i], inv_temp));
+  }
+  if (!use_min_p) return;
+  // p_i < min_p * max p  <=>  exp(z_i - m) < min_p
+  __shared__ float s_max[kPenThreads / 32];
+  m = warp_max(m);
+  if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = -INFINITY;
+  for (int w = 0; w < kPenThreads / 32; ++w) m = fmaxf(m, s_max[w]);
+  // each thread reads back the elements it wrote in pass 1 (same index mapping)
+#pragma unroll 2
+  for (int j = threadIdx.x; j < V4; j += kPenThreads) {
+    float4 l = row4[j];
+    if (expf(__fmul_rn(l.x, inv_temp) - m) < min_p) l.x = -INFINITY;
+    if (expf(__fmul_rn(l.y, inv_temp) - m) < min_p) l.y = -INFINITY;
+    if (expf(__fmul_rn(l.z, inv_temp) - m) < min_p) l.z = -INFINITY;
+    if (expf(__fmul_rn(l.w, inv_temp) - m) < min_p) l.w = -INFINITY;
+    row4[j] = l;
+  }
+  for (int i = (V4 << 2) + threadIdx.x; i < V; i += kPenThreads)
+    if (expf(__fmul_rn(row[i], inv_temp) - m) < min_p) row[i] = -INFINITY;
+}
+
 }  // namespace
 }  // namespace prl
 
@@ -760,6 +866,20 @@ extern "C" int prl_ban_min_tokens(float* logits, int32_t B, int32_t V, const int
                 ban_stride);
   PRL_CUDA(launch_pdl(ban_min_tokens_kernel, dim3((B + 3) / 4), dim3(128), 0, (cudaStream_t)st, logits, (int)B, (int)V,
                       gen_count, min_tokens, ban_ids, (int)ban_stride, n_ban));
+  PRL_LAUNCH_CHECK();
+  return PRL_OK;
+}
+
+extern "C" int prl_apply_penalties(const prl_penalties* p, prl_stream_t st) {
+  PRL_CHECK_ARG(p != nullptr, "prl_apply_penalties: NULL argument");
+  PRL_CHECK_ARG(p->B >= 1 && p->V >= 1 && p->prompt_stride >= 1 && p->out_stride >= 1,
+                "prl_apply_penalties: bad shape (B=%d, V=%d, prompt_stride=%d, out_stride=%d)", p->B, p->V,
+                p->prompt_stride, p->out_stride);
+  PRL_CHECK_ARG(p->logits && p->presence && p->frequency && p->repetition && p->min_p && p->inv_temp && p->greedy &&
+                    p->prompt_buf && p->prompt_len && p->out_ids && p->gen_count && p->counts && p->prompt_mask &&
+                    p->seen,
+                "prl_apply_penalties: NULL field");
+  PRL_CUDA(launch_pdl(penalties_kernel, dim3(p->B), dim3(kPenThreads), 0, (cudaStream_t)st, *p));
   PRL_LAUNCH_CHECK();
   return PRL_OK;
 }

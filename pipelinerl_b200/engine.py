@@ -39,6 +39,10 @@ class SamplingParams:
     min_tokens: int = 0                    # no stop (eos, stop ids, strings) before this many outputs; eos / stop ids banned
     include_stop_str_in_output: bool = False   # vLLM's defaults; with stop strings only the pairs (True, False) and
     skip_special_tokens: bool = True           # (False, True) are implemented
+    presence_penalty: float = 0.0          # logit -= presence_penalty when the id is among the outputs so far
+    frequency_penalty: float = 0.0         # logit -= frequency_penalty * (times the id is among the outputs so far)
+    repetition_penalty: float = 1.0        # ids in the prompt or outputs: positive logits / it, the others * it
+    min_p: float = 0.0                     # drop ids with probability < min_p * the largest (after the temperature)
 
 
 def truncation_params(params: dict, greedy: bool = False) -> tuple[int, float]:
@@ -57,6 +61,39 @@ def truncation_params(params: dict, greedy: bool = False) -> tuple[int, float]:
     if greedy:
         return -1, 1.0
     return int(top_k), float(top_p)
+
+
+PENALTY_DEFAULTS = {"presence_penalty": 0.0, "frequency_penalty": 0.0, "repetition_penalty": 1.0, "min_p": 0.0}
+
+
+def penalty_params(params: dict, greedy: bool = False) -> tuple[float, float, float, float]:
+    """(presence_penalty, frequency_penalty, repetition_penalty, min_p) of a request body / `llm.parameters`, validated
+    as vLLM's SamplingParams._verify_args validates them: presence and frequency in [-2, 2], repetition > 0, min_p in
+    [0, 1]; a missing or None value is the default.  Non-finite values are refused as well (vLLM lets an infinite or NaN
+    repetition_penalty through, which turns the row's logits into NaN).  Greedy requests get min_p 0: vLLM resets it
+    at temperature 0 after validating it; the penalties stay, as they change the argmax.  Raises ValueError."""
+    out = []
+    for name, default in PENALTY_DEFAULTS.items():
+        v = params.get(name)
+        v = default if v is None else v
+        if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v):
+            raise ValueError(f"{name} must be a finite number, got {v!r}")
+        out.append(float(v))
+    presence, frequency, repetition, min_p = out
+    if not -2.0 <= presence <= 2.0:
+        raise ValueError(f"presence_penalty must be in [-2, 2], got {presence}.")
+    if not -2.0 <= frequency <= 2.0:
+        raise ValueError(f"frequency_penalty must be in [-2, 2], got {frequency}.")
+    if repetition <= 0.0:
+        raise ValueError(f"repetition_penalty must be greater than zero, got {repetition}.")
+    if not 0.0 <= min_p <= 1.0:
+        raise ValueError(f"min_p must be in [0, 1], got {min_p}.")
+    return presence, frequency, repetition, 0.0 if greedy else min_p
+
+
+def requested_penalties(penalties: tuple[float, float, float, float]) -> set[str]:
+    """The penalty / min_p features a validated `penalty_params` tuple asks for."""
+    return {name for (name, default), v in zip(PENALTY_DEFAULTS.items(), penalties) if v != default}
 
 
 def stop_token_ids_param(params: dict) -> tuple[int, ...]:
@@ -342,6 +379,10 @@ class DecodeEngine:
         self.ban_rows = torch.zeros(B, self.ban_stride, **i32)
         self.n_ban = torch.zeros(B, **i32)
         self._min_slots: set[int] = set()
+        # penalties and min_p per slot: the rows and the count / prompt-mask state are allocated by the first request
+        # that asks for one, and the kernel runs only while some slot in _pen_slots uses them
+        self._pen = None
+        self._pen_slots: set[int] = set()
         self._temperature, self._greedy, self._ignore_eos = 1.0, False, False
         self._graphs: dict[int, torch.cuda.CUDAGraph] = {}
         # ---- chunked prefill + prefix sharing (GRPO attempts share their prompt) ----
@@ -379,6 +420,11 @@ class DecodeEngine:
     @property
     def supports_min_tokens(self) -> bool:
         """The min_tokens ban writes -inf into the logits, which only the unfused head keeps in HBM."""
+        return not self.fused_head
+
+    @property
+    def supports_penalties(self) -> bool:
+        """Presence / frequency / repetition penalties and min_p rewrite the logits in HBM: unfused head only."""
         return not self.fused_head
 
     # engine-wide sampling defaults: assigning one overwrites every slot (benches, tools, single-tenant tests)
@@ -464,6 +510,36 @@ class DecodeEngine:
             _lib.check(self.lib.prl_ban_min_tokens(self.logits.data_ptr(), self.B, self.cfg.head_rows,
                                                    self.gen_count.data_ptr(), self.min_tokens_rows.data_ptr(),
                                                    self.ban_rows.data_ptr(), self.ban_stride, self.n_ban.data_ptr(), st))
+
+    def _penalty_state(self) -> _lib.Penalties:
+        """The per-slot penalty rows and the kernel's argument struct, allocated on first use: an output count row
+        (int32 [B, V]), a prompt bitmask (uint32 [B, ceil(V / 32)]) and the outputs already counted (-1: reset)."""
+        if self._pen is None:
+            d, B, V = self.dev, self.B, self.cfg.head_rows
+            self.presence_rows = torch.zeros(B, dtype=torch.float32, device=d)
+            self.frequency_rows = torch.zeros(B, dtype=torch.float32, device=d)
+            self.repetition_rows = torch.ones(B, dtype=torch.float32, device=d)
+            self.min_p_rows = torch.zeros(B, dtype=torch.float32, device=d)
+            self.pen_counts = torch.zeros(B, V, dtype=torch.int32, device=d)
+            self.pen_prompt_mask = torch.zeros(B, (V + 31) // 32, dtype=torch.int32, device=d)
+            self.pen_seen = torch.full((B,), -1, dtype=torch.int32, device=d)
+            p = self._pen = _lib.Penalties()
+            p.logits, p.B, p.V = self.logits.data_ptr(), B, V
+            p.presence, p.frequency = self.presence_rows.data_ptr(), self.frequency_rows.data_ptr()
+            p.repetition, p.min_p = self.repetition_rows.data_ptr(), self.min_p_rows.data_ptr()
+            p.inv_temp, p.greedy = self.inv_temp_rows.data_ptr(), self.greedy_rows.data_ptr()
+            p.prompt_buf, p.prompt_stride, p.prompt_len = (self.prompt_buf.data_ptr(), self.prompt_stride,
+                                                           self.prompt_len.data_ptr())
+            p.out_ids, p.out_stride, p.gen_count = self.out_ids.data_ptr(), self.max_new, self.gen_count.data_ptr()
+            p.counts, p.prompt_mask = self.pen_counts.data_ptr(), self.pen_prompt_mask.data_ptr()
+            p.seen = self.pen_seen.data_ptr()
+        return self._pen
+
+    def _apply_penalties(self, st: int) -> None:
+        """vLLM's penalties, then min_p after the temperature, on the rows of the slots that ask for them: between the
+        min_tokens ban and the sampler, outside the CUDA graph."""
+        if self._pen_slots:
+            _lib.check(self.lib.prl_apply_penalties(C.byref(self._pen), st))
 
     # ------------------------------------------------------------------------------------------
     def _gemm(self, w_name: str, x: torch.Tensor, n: int, k: int, split: int, out: torch.Tensor, lo: str | None = None,
@@ -565,6 +641,7 @@ class DecodeEngine:
             self._advance(st)
             return
         self._ban_min_tokens(st)
+        self._apply_penalties(st)
         if self._truncated_slots:
             _lib.check(lib.prl_sample_logprob_topkp_rows(self.logits.data_ptr(), self.B, self.cfg.head_rows,
                                                          self.inv_temp_rows.data_ptr(), self.greedy_rows.data_ptr(),
@@ -941,6 +1018,10 @@ class DecodeEngine:
         if min_tokens and not self.supports_min_tokens:
             raise ValueError(f"min_tokens is not implemented by this engine ({type(self).__name__}, "
                              f"fused_head={self.fused_head})")
+        penalties = penalty_params({k: getattr(params, k) for k in PENALTY_DEFAULTS}, greedy=params.greedy)
+        if requested_penalties(penalties) and not self.supports_penalties:
+            raise ValueError(f"{' / '.join(sorted(requested_penalties(penalties)))} is not implemented by this engine "
+                             f"({type(self).__name__}, fused_head={self.fused_head})")
         if not self.can_admit(n, params.max_tokens):
             raise RuntimeError("engine full")
         req = Request(self._next_id, list(prompt_ids), params, model_version=model_version)
@@ -1024,6 +1105,12 @@ class DecodeEngine:
             if ban:
                 self.ban_rows[slot, :len(ban)].copy_(torch.tensor(ban, dtype=torch.int32), non_blocking=True)
             self._min_slots.add(slot)
+        if requested_penalties(penalties):         # other slots keep the defaults (reset at harvest)
+            self._penalty_state()
+            self.presence_rows[slot], self.frequency_rows[slot], self.repetition_rows[slot], self.min_p_rows[slot] = \
+                penalties
+            self.pen_seen[slot] = -1               # the kernel resets the slot's counts and prompt mask
+            self._pen_slots.add(slot)
         self.tokens[slot] = prompt_ids[start]
         self.positions[slot] = start
         self.seq_lens[slot] = start + 1
@@ -1062,6 +1149,10 @@ class DecodeEngine:
             if slot in self._min_slots:
                 self._min_slots.discard(slot)
                 self.min_tokens_rows[slot] = 0
+            if slot in self._pen_slots:
+                self._pen_slots.discard(slot)
+                self.presence_rows[slot], self.frequency_rows[slot], self.repetition_rows[slot], self.min_p_rows[slot] = \
+                    PENALTY_DEFAULTS.values()
             self.block_table[slot].zero_()
             self.finished[slot] = 0
             if slot in self._truncated_slots:

@@ -7,7 +7,8 @@ at this shim instead of a vLLM server (SURVEY §8b "wire format"):
 
   POST /v1/chat/completions   request fields the reference sends (async_llm.py:96-131): model, messages, logprobs,
                               include_stop_str_in_output, skip_special_tokens, tools?, max_tokens?, chat_template_kwargs?
-                              + llm.parameters (temperature, top_p, top_k ...);  response fields it reads (:173-207):
+                              + llm.parameters (temperature, top_p, top_k, stop, min_tokens, presence_penalty,
+                              frequency_penalty, repetition_penalty, min_p ...);  response fields it reads (:173-207):
                               choices[0].message.{content, tool_calls}, choices[0].logprobs.content[i].{token, logprob}
                               with token = "token_id:<id>" (--return-tokens-as-token-ids), choices[0].finish_reason in
                               {stop, length}, usage.{prompt_tokens, completion_tokens}
@@ -20,10 +21,12 @@ at this shim instead of a vLLM server (SURVEY §8b "wire format"):
 top_k / top_p are served when the engine lists them in `engine.sampling_features` (the unfused single-GPU DecodeEngine:
 vLLM's truncation rule, with the logprob of the truncated distribution), and stop_token_ids when the engine sets
 `supports_stop_token_ids` (every DecodeEngine; the choice then reports vLLM's `stop_reason`, the stop id that ended it).
-They are validated as vLLM validates them.
-Sampling features the engine does not implement (truncation on the fused-head or TP engines, n > 1, streaming) are
-rejected with 400 rather than silently ignored.  Host code only: the engine behind it is the CUDA DecodeEngine (no CPU
-fallback).
+Stop strings and min_tokens are served when the engine sets `supports_stop_strings` / `supports_min_tokens`, and
+presence_penalty, frequency_penalty, repetition_penalty and min_p when it sets `supports_penalties` (the unfused
+single-GPU DecodeEngine).  All of them are validated as vLLM validates them.
+Sampling features the engine does not implement (truncation, min_tokens, penalties or min_p on the fused-head or TP
+engines, n > 1, streaming) are rejected with 400 rather than silently ignored.  Host code only: the engine behind it is
+the CUDA DecodeEngine (no CPU fallback).
 """
 from __future__ import annotations
 
@@ -35,8 +38,8 @@ from typing import Any
 
 from aiohttp import web
 
-from .engine import (SamplingParams, check_stop_flags, min_tokens_param, requested_truncation, stop_strings_param,
-                     stop_token_ids_param, truncation_params)
+from .engine import (SamplingParams, check_stop_flags, min_tokens_param, penalty_params, requested_penalties,
+                     requested_truncation, stop_strings_param, stop_token_ids_param, truncation_params)
 from .serving import engine_features
 
 
@@ -120,6 +123,7 @@ class HttpShim:
             stop = stop_strings_param(body)
             min_tokens = min_tokens_param(body, max_tokens)
             check_stop_flags(stop, include, skip)
+            penalties = penalty_params(body, greedy=temperature <= 0)
         except ValueError as e:
             return self._bad(str(e))
         engine = getattr(self.server, "engine", None)
@@ -133,11 +137,15 @@ class HttpShim:
             return self._bad("stop strings are not implemented by this engine")
         if min_tokens and "min_tokens" not in features:
             return self._bad("min_tokens is not implemented by this engine")
+        missing = requested_penalties(penalties) - features
+        if missing:
+            return self._bad(f"{' / '.join(sorted(missing))} is not implemented by this engine")
         if int(body.get("n", 1)) != 1 or body.get("stream"):
             return self._bad("n > 1 and streaming are not implemented")
         sp = SamplingParams(max_tokens=max_tokens, temperature=temperature if temperature > 0 else 1.0,
                             greedy=temperature <= 0, top_k=top_k, top_p=top_p, stop_token_ids=stop_ids, stop=stop,
                             min_tokens=min_tokens, include_stop_str_in_output=include, skip_special_tokens=skip)
+        sp.presence_penalty, sp.frequency_penalty, sp.repetition_penalty, sp.min_p = penalties
         try:
             if stop_ids:
                 engine.stop_row(sp)        # ids outside the vocabulary, or more than a slot's stop row holds

@@ -13,7 +13,7 @@ import queue
 import threading
 from dataclasses import dataclass
 
-from .engine import DecodeEngine, Request, SamplingParams
+from .engine import PENALTY_DEFAULTS, DecodeEngine, Request, SamplingParams
 
 _REGISTRY: dict[str, "EngineServer"] = {}
 
@@ -40,9 +40,12 @@ def sampling_features(base_url: str) -> frozenset:
 
 def engine_features(engine) -> frozenset:
     """An engine's `sampling_features`, plus "stop_token_ids" when it sets `supports_stop_token_ids`, "stop" (stop
-    strings) when it sets `supports_stop_strings` and "min_tokens" when it sets `supports_min_tokens`."""
+    strings) when it sets `supports_stop_strings`, "min_tokens" when it sets `supports_min_tokens` and the four names
+    of PENALTY_DEFAULTS (presence / frequency / repetition penalties, min_p) when it sets `supports_penalties`."""
     extra = {name for name, attr in (("stop_token_ids", "supports_stop_token_ids"), ("stop", "supports_stop_strings"),
                                      ("min_tokens", "supports_min_tokens")) if getattr(engine, attr, False)}
+    if getattr(engine, "supports_penalties", False):
+        extra |= set(PENALTY_DEFAULTS)
     return frozenset(getattr(engine, "sampling_features", frozenset())) | extra
 
 

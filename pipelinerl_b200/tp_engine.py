@@ -33,6 +33,8 @@ class TPDecodeEngine(DecodeEngine):
     # neither stop strings nor min_tokens: add_request refuses both here
     supports_stop_strings = False
     supports_min_tokens = False
+    # no penalties or min_p either: no rank holds a whole row of logits
+    supports_penalties = False
 
     def __init__(self, full_cfg: ModelConfig, arena: ParamArena, tp_rank: int, tp_size: int, group=None, **kw):
         import torch.distributed as dist
